@@ -80,6 +80,12 @@ _SIGS = {
     "b200z_zip_comment": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     "b200z_zip_extract": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]),
+    "b200z_zip_crypt_info": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                                       C.POINTER(C.c_uint32)]),
+    "b200z_zip_extract_password": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]),
+    "b200z_zip_aes_encrypt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
+                                        C.c_void_p, C.c_void_p]),
     "b200z_bzip2_decode_shard": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,
                                            C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_bzip2_encode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -19,6 +19,11 @@
 
 #include "b200z_internal.h"
 #include "bzip2_enc.h"
+#ifdef B200Z_EMU
+// The CPU emulation build of the library compiles the generated copies of the .cu files it lists; the encrypted-member
+// kernels come in here (zip_crypt_kernels.cu launches through ZC_LAUNCH, which both compilers take).
+#include "zip_crypt_kernels.cu"
+#endif
 
 namespace b200z {
 
@@ -108,7 +113,7 @@ struct Ctx {
   cudaStream_t stream = nullptr, s_h2d = nullptr, s_d2h = nullptr;
   static const int kCompStreams = 8;
   cudaStream_t s_comp[kCompStreams] = {};
-  DevBuf d_in, d_out, d_ws, d_meta, d_small, d_bz, d_tok;
+  DevBuf d_in, d_out, d_ws, d_meta, d_small, d_bz, d_tok, d_crypt;
   PinBuf h_meta;
 };
 static Ctx g;
@@ -1871,15 +1876,19 @@ extern "C" int b200z_zip_comment(const uint8_t *z, size_t len, uint64_t *off, ui
   return B200Z_OK;
 }
 
-extern "C" int b200z_zip_extract(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
-                                 size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
-                                 int32_t *status, uint32_t flags) {
-  int rc = require_init();
-  if (rc) return rc;
-  if (n == 0) return B200Z_OK;
-  if (!entries || !out_off || !out_room || !out_len || !status) return B200Z_E_ARG;
-  std::lock_guard<std::mutex> lk(g.mu);
-  CU(cudaSetDevice(g.device));
+// Encrypted members after decryption (b200z_zip_extract_password): their plaintext sits in g.d_in behind the archive, and
+// the entries handed to zip_extract_core point there.
+struct ZipPlain {
+  size_t staged;                                // bytes of g.d_in in use: the archive, then the plaintext area
+  const std::vector<const uint8_t *> *bz_src;   // per member: host copy of a decrypted bzip2 member, or null
+};
+
+// ZipFile.getStream for all members (g.mu held).  pl == nullptr: the archive is not staged yet and `len` is its size;
+// otherwise `len` = pl->staged and everything is in g.d_in already.
+static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
+                            size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
+                            int32_t *status, uint32_t flags, const ZipPlain *pl) {
+  int rc = B200Z_OK;
   // members: deflate -> one inflate batch; stored (and unknown methods, which the reference treats as stored,
   // zip_file.dart:83) -> device copies; bzip2 -> one stream each, afterwards
   std::vector<uint64_t> u_in_off, u_out_off;
@@ -1932,8 +1941,10 @@ extern "C" int b200z_zip_extract(const uint8_t *z, size_t len, const b200z_zip_e
   }
   const bool any_dev = hi > lo;
   if (any_dev || !u_idx.empty()) {
-    rc = stage_input(z, len);
-    if (rc) return rc;
+    if (!pl) {
+      rc = stage_input(z, len);
+      if (rc) return rc;
+    }
     CU(cudaMemsetAsync((uint8_t *)g.d_in.p + len, 0, 64, g.stream));
     CU(g.d_out.reserve((hi ? hi : 1) + 64));
   }
@@ -2078,11 +2089,362 @@ extern "C" int b200z_zip_extract(const uint8_t *z, size_t len, const b200z_zip_e
   for (size_t i : bz_idx) {  // BZip2Decoder().decodeStream(_rawContent, output) (zip_file.dart:189-192,239-245)
     const b200z_zip_entry &e = entries[i];
     size_t got = 0;
-    rc = bzip2_decode_impl(z + e.data_off, (size_t)e.comp_size, 0, out + out_off[i], (size_t)out_room[i], &got);
+    const uint8_t *src = pl && (*pl->bz_src)[i] ? (*pl->bz_src)[i] : z + e.data_off;
+    rc = bzip2_decode_impl(src, (size_t)e.comp_size, 0, out + out_off[i], (size_t)out_room[i], &got);
     out_len[i] = got;
     status[i] = rc == B200Z_OK ? B200Z_U_DONE : rc == B200Z_E_NOSPC ? B200Z_U_NOSPC : rc == B200Z_E_THROW ? B200Z_U_THROW : B200Z_U_STOP;
   }
   return B200Z_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Encrypted ZIP members (zip_file.dart:98-130 read, :164-216 getStream, :260-359 ZipCrypto / AES)
+// ---------------------------------------------------------------------------------------------
+// ZipFile.read :98-130: flag bit 0 means ZipCrypto, unless the LOCAL extra field is longer than 2 bytes and holds id 0x9901.
+// The scan reads 16-bit ids at 2-byte steps and never skips the payload of another id (the reference's loop, kept as is);
+// a read past the end of the extra field throws there.
+static int zip_crypt_info_impl(const uint8_t *z, size_t len, const b200z_zip_entry *e, uint32_t *mode, uint32_t *strength,
+                               uint32_t *method) {
+  *mode = B200Z_ZIP_CRYPT_NONE;
+  *strength = 0;
+  *method = e->method;
+  if (!e->has_data || !(e->flags & 1u)) return B200Z_OK;
+  *mode = B200Z_ZIP_CRYPT_ZIPCRYPTO;
+  const uint64_t x0 = e->name_off + e->name_len;
+  if (x0 > e->data_off || e->data_off > len) {
+    set_err("zip_crypt_info: entry does not lie inside the archive");
+    return B200Z_E_ARG;
+  }
+  const uint64_t xl = e->data_off - x0;
+  if (xl <= 2) return B200Z_OK;
+  const uint8_t *x = z + x0;
+  uint64_t q = 0;
+  bool past = false;  // a read ran over the end of the extra field
+  while (q < xl && !past) {
+    if (xl - q < 2) {
+      past = true;
+      break;
+    }
+    const uint32_t id = le16(x + q);
+    q += 2;
+    if (id != 0x9901u) continue;
+    q += 4;                             // dataSize, vendorVersion
+    q = q + 2 > xl ? (q > xl ? q : xl) : q + 2;  // readString(size: 2): readBytes hands out what is there
+    if (q > xl || xl - q < 3) {        // strength (1 byte) and compression method (2 bytes)
+      past = true;
+      break;
+    }
+    *mode = B200Z_ZIP_CRYPT_AES;
+    *strength = x[q];
+    *method = le16(x + q + 1);
+    q += 3;
+  }
+  if (past) {
+    set_err("zip: the scan of the AES extra field reads past its end (Dart: RangeError)");
+    return B200Z_E_THROW;
+  }
+  return B200Z_OK;
+}
+
+static double g_crypt_ms[4];  // last call: PBKDF2, CTR, MAC, ZipCrypto kernel times (b200z_debug_zip_crypt_ms)
+
+struct CryptEvents {  // CUDA events around the kernels: PBKDF2 [0,1], CTR [2,3], MAC [2,5] (it may start at 2), ZipCrypto [6,7]
+  cudaEvent_t ev[8] = {};
+  bool used[4] = {};
+  CryptEvents() {
+    for (auto &e : ev) cudaEventCreate(&e);
+  }
+  ~CryptEvents() {
+    for (auto &e : ev)
+      if (e) cudaEventDestroy(e);
+  }
+};
+
+static inline uint32_t aes_salt_len(uint32_t strength) { return strength == 1 ? 8 : strength == 2 ? 12 : 16; }
+
+// tiles of k_zip_aes_ctr over the members with len > 0
+static void ctr_tiles(const std::vector<ZipAesMember> &m, std::vector<ZipCtrTile> &t) {
+  const uint64_t tb = zip_ctr_tile_blocks();
+  t.clear();
+  for (size_t k = 0; k < m.size(); ++k) {
+    const uint64_t blocks = (m[k].len + 15) / 16;
+    for (uint64_t b = 0; b < blocks; b += tb) t.push_back(ZipCtrTile{b, (uint32_t)k, 0});
+  }
+}
+
+// device layout of the crypt metadata in g.d_crypt
+struct CryptLayout {
+  size_t members, dk, rk, ver, mac, tiles, zc, bytes;
+  CryptLayout(size_t na, size_t nt, size_t nz) {
+    size_t o = 0;
+    members = o; o = align_up(o + na * sizeof(ZipAesMember), 256);
+    dk = o;      o = align_up(o + na * 80, 256);
+    rk = o;      o = align_up(o + na * 240, 256);
+    ver = o;     o = align_up(o + na * 2, 256);
+    mac = o;     o = align_up(o + na * 10, 256);
+    tiles = o;   o = align_up(o + nt * sizeof(ZipCtrTile), 256);
+    zc = o;      o = align_up(o + nz * sizeof(ZipCryptoMember), 256);
+    bytes = o + 256;
+  }
+};
+
+static int zip_extract_crypt(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
+                             size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
+                             int32_t *status, uint32_t flags, const uint8_t *pw, size_t pw_len) {
+  // 1. which members are encrypted how, and where their plaintext goes: the plaintext area starts behind the archive in
+  //    g.d_in, every member is followed by >= 64 zero bytes (the inflate look-ahead reads zeros, as the oracle's does)
+  std::vector<b200z_zip_entry> ve(entries, entries + n);
+  std::vector<int32_t> forced(n, 1);  // 1: none; otherwise the member's final status (out_len 0)
+  std::vector<ZipAesMember> aes;
+  std::vector<uint32_t> aes_idx;
+  std::vector<ZipCryptoMember> zc;
+  size_t p = align_up(len + 64, 256);
+  for (size_t i = 0; i < n; ++i) {
+    const b200z_zip_entry &e = entries[i];
+    if (!e.has_data || !(e.flags & 1u)) continue;
+    if (e.data_off > len || e.comp_size > len - e.data_off) {
+      set_err("zip_extract: entry %zu lies outside the buffers", i);
+      return B200Z_E_ARG;
+    }
+    uint32_t mode, strength, method;
+    const int ci = zip_crypt_info_impl(z, len, &e, &mode, &strength, &method);
+    if (ci == B200Z_E_ARG) return ci;
+    ve[i].flags &= ~1u;
+    ve[i].method = method;
+    if (ci != B200Z_OK) {  // ZipFile.read throws for this member
+      forced[i] = B200Z_U_THROW;
+      ve[i].has_data = 0;
+      continue;
+    }
+    if (e.comp_size == 0) continue;  // :170-171: an empty member is not decrypted; it is an empty member of its method
+    uint64_t plen;
+    if (mode == B200Z_ZIP_CRYPT_ZIPCRYPTO) {
+      if (e.comp_size < 12) {  // _decodeZipCrypto: readByte past the end
+        forced[i] = B200Z_U_THROW;
+        ve[i].has_data = 0;
+        continue;
+      }
+      plen = e.comp_size - 12;
+      zc.push_back(ZipCryptoMember{e.data_off, p, e.comp_size});
+    } else {
+      const uint32_t sl = aes_salt_len(strength);
+      if (e.comp_size < sl + 12 || pw_len == 0) {  // readBytes(input.length - 10) < 0; deriveKey('') -> sublist throws
+        forced[i] = B200Z_U_THROW;
+        ve[i].has_data = 0;
+        continue;
+      }
+      plen = e.comp_size - sl - 12;
+      ZipAesMember m;
+      memset(&m, 0, sizeof m);
+      m.src_off = e.data_off + sl + 2;
+      m.dst_off = p;
+      m.len = plen;
+      m.salt_len = sl;
+      m.key_len = 2 * sl;
+      memcpy(m.salt, z + e.data_off, sl);
+      aes.push_back(m);
+      aes_idx.push_back((uint32_t)i);
+    }
+    ve[i].data_off = p;
+    ve[i].comp_size = plen;
+    p = align_up(p + plen + 64, 256);
+  }
+  if (aes.empty() && zc.empty()) {
+    int rc = zip_extract_core(z, len, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr);
+    for (size_t i = 0; i < n && rc == B200Z_OK; ++i)
+      if (forced[i] != 1) {
+        status[i] = forced[i];
+        out_len[i] = 0;
+      }
+    return rc;
+  }
+  // 2. stage the archive once; the plaintext area is zeroed
+  const size_t staged = p;
+  CU(g.d_in.reserve(staged + 64));
+  uint8_t *d_base = (uint8_t *)g.d_in.p;
+  CU(cudaMemcpyAsync(d_base, z, len, cudaMemcpyHostToDevice, g.stream));
+  CU(cudaMemsetAsync(d_base + len, 0, staged + 64 - len, g.stream));
+  std::vector<ZipCtrTile> tiles;
+  const uint32_t na = (uint32_t)aes.size(), nz = (uint32_t)zc.size();
+  // tiles are counted for every member: the verifier check below can only shrink the list
+  ctr_tiles(aes, tiles);
+  const CryptLayout cl(na, tiles.size(), nz);
+  CU(g.d_crypt.reserve(cl.bytes));
+  uint8_t *dc = (uint8_t *)g.d_crypt.p;
+  CryptEvents ev;
+  std::vector<uint8_t> macs(na * 10);
+  cudaStream_t s_mac = g.s_comp[0];
+  // 3. AES: key derivation, verifier check on the host, then the MAC (second stream) and the CTR pass
+  if (na) {
+    ZipHmacPads pads;
+    zip_hmac_pads(pw, pw_len, &pads);
+    CU(cudaMemcpyAsync(dc + cl.members, aes.data(), na * sizeof(ZipAesMember), cudaMemcpyHostToDevice, g.stream));
+    CU(cudaEventRecord(ev.ev[0], g.stream));
+    CU(zip_launch_pbkdf2((const ZipAesMember *)(dc + cl.members), na, pads, dc + cl.dk, (uint32_t *)(dc + cl.rk), dc + cl.ver,
+                         g.stream));
+    CU(cudaEventRecord(ev.ev[1], g.stream));
+    ev.used[0] = true;
+    std::vector<uint8_t> ver(na * 2);
+    CU(cudaMemcpyAsync(ver.data(), dc + cl.ver, na * 2, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+    bool any_bad = false;
+    for (uint32_t k = 0; k < na; ++k) {
+      const b200z_zip_entry &e = entries[aes_idx[k]];
+      if (memcmp(ver.data() + 2 * k, z + e.data_off + aes[k].salt_len, 2) != 0) {  // Exception('password error')
+        forced[aes_idx[k]] = B200Z_ZIP_BAD_PASSWORD;
+        ve[aes_idx[k]].has_data = 0;
+        aes[k].len = 0;
+        any_bad = true;
+      }
+    }
+    if (any_bad) {
+      ctr_tiles(aes, tiles);
+      CU(cudaMemcpyAsync(dc + cl.members, aes.data(), na * sizeof(ZipAesMember), cudaMemcpyHostToDevice, g.stream));
+    }
+    CU(cudaMemcpyAsync(dc + cl.tiles, tiles.data(), tiles.size() * sizeof(ZipCtrTile), cudaMemcpyHostToDevice, g.stream));
+    CU(cudaEventRecord(ev.ev[2], g.stream));  // the MAC stream starts once the key material and the member list are there
+    CU(cudaStreamWaitEvent(s_mac, ev.ev[2], 0));
+    CU(zip_launch_hmac((const ZipAesMember *)(dc + cl.members), na, dc + cl.dk, d_base, false, dc + cl.mac, s_mac));
+    CU(cudaEventRecord(ev.ev[5], s_mac));
+    ev.used[2] = true;
+    CU(zip_launch_aes_ctr((const ZipAesMember *)(dc + cl.members), (const uint32_t *)(dc + cl.rk), (const ZipCtrTile *)(dc + cl.tiles),
+                          (uint32_t)tiles.size(), d_base, g.stream));
+    CU(cudaEventRecord(ev.ev[3], g.stream));
+    ev.used[1] = true;
+  }
+  // 4. ZipCrypto
+  if (nz) {
+    uint32_t keys[3];
+    zipcrypto_keys(pw, pw_len, keys);
+    CU(cudaMemcpyAsync(dc + cl.zc, zc.data(), nz * sizeof(ZipCryptoMember), cudaMemcpyHostToDevice, g.stream));
+    CU(cudaEventRecord(ev.ev[6], g.stream));
+    CU(zip_launch_zipcrypto((const ZipCryptoMember *)(dc + cl.zc), nz, keys, d_base, g.stream));
+    CU(cudaEventRecord(ev.ev[7], g.stream));
+    ev.used[3] = true;
+  }
+  // 5. bzip2 members are decoded from host memory (bzip2_decode_impl): their plaintext comes back first
+  std::vector<const uint8_t *> bz_src(n, nullptr);
+  std::vector<std::vector<uint8_t>> bz_keep;
+  for (size_t i = 0; i < n; ++i) {
+    if (!ve[i].has_data || !(entries[i].flags & 1u) || ve[i].method != 12 || ve[i].data_off < len) continue;
+    bz_keep.emplace_back(ve[i].comp_size + 1);
+    CU(cudaMemcpyAsync(bz_keep.back().data(), d_base + ve[i].data_off, ve[i].comp_size, cudaMemcpyDeviceToHost, g.stream));
+    bz_src[i] = bz_keep.back().data();
+  }
+  if (!bz_keep.empty()) CU(cudaStreamSynchronize(g.stream));
+  // 6. everything else sees the decrypted members as ranges of the staged buffer
+  const ZipPlain pl{staged, &bz_src};
+  int rc = zip_extract_core(z, staged, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, &pl);
+  if (rc) {
+    cudaStreamSynchronize(s_mac);
+    return rc;
+  }
+  // 7. the MACs: HMAC-SHA1 of the ciphertext, first 10 bytes, against the 10 bytes that end the member
+  if (na) {
+    CU(cudaStreamSynchronize(s_mac));
+    CU(cudaMemcpy(macs.data(), dc + cl.mac, na * 10, cudaMemcpyDeviceToHost));
+    for (uint32_t k = 0; k < na; ++k) {
+      const uint32_t i = aes_idx[k];
+      if (forced[i] != 1) continue;
+      const b200z_zip_entry &e = entries[i];
+      if (memcmp(macs.data() + 10 * k, z + e.data_off + e.comp_size - 10, 10) != 0) forced[i] = B200Z_ZIP_BAD_MAC;
+    }
+  }
+  CU(cudaStreamSynchronize(g.stream));
+  {
+    float ms = 0;
+    g_crypt_ms[0] = ev.used[0] && cudaEventElapsedTime(&ms, ev.ev[0], ev.ev[1]) == cudaSuccess ? ms : 0.0;
+    g_crypt_ms[1] = ev.used[1] && cudaEventElapsedTime(&ms, ev.ev[2], ev.ev[3]) == cudaSuccess ? ms : 0.0;
+    g_crypt_ms[2] = ev.used[2] && cudaEventElapsedTime(&ms, ev.ev[2], ev.ev[5]) == cudaSuccess ? ms : 0.0;
+    g_crypt_ms[3] = ev.used[3] && cudaEventElapsedTime(&ms, ev.ev[6], ev.ev[7]) == cudaSuccess ? ms : 0.0;
+  }
+  for (size_t i = 0; i < n; ++i)
+    if (forced[i] != 1) {
+      status[i] = forced[i];
+      out_len[i] = 0;
+    }
+  return B200Z_OK;
+}
+
+extern "C" int b200z_zip_crypt_info(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *entry, uint32_t *mode,
+                                    uint32_t *aes_strength, uint32_t *method) {
+  if (!entry || !mode || !aes_strength || !method || (!zip && zip_len)) return B200Z_E_ARG;
+  return zip_crypt_info_impl(zip, zip_len, entry, mode, aes_strength, method);
+}
+
+extern "C" int b200z_zip_extract_password(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
+                                          size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
+                                          int32_t *status, uint32_t flags, const uint8_t *password, size_t password_len) {
+  int rc = require_init();
+  if (rc) return rc;
+  if (n == 0) return B200Z_OK;
+  if (!entries || !out_off || !out_room || !out_len || !status) return B200Z_E_ARG;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  if (!password) return zip_extract_core(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr);
+  return zip_extract_crypt(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, password, password_len);
+}
+
+extern "C" int b200z_zip_extract(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
+                                 size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
+                                 int32_t *status, uint32_t flags) {
+  return b200z_zip_extract_password(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr, 0);
+}
+
+// ZipEncoder._encryptCompressedData (zip_encoder.dart:166-183) for n members at once: AES-256, CTR in place, then the MAC
+// of the ciphertext.  One copy of data[0, max(off + len)) to the device and one back.
+extern "C" int b200z_zip_aes_encrypt(uint8_t *data, const uint64_t *off, const uint64_t *len, size_t n, const uint8_t *salts,
+                                     const uint8_t *password, size_t password_len, uint8_t *pwd_verify, uint8_t *mac) {
+  int rc = require_init();
+  if (rc) return rc;
+  if (n == 0) return B200Z_OK;
+  if (!data || !off || !len || !salts || !password || !pwd_verify || !mac) return B200Z_E_ARG;
+  if (password_len == 0) {
+    set_err("zip_aes_encrypt: empty password (Dart: ZipFile.deriveKey returns an empty list, sublist throws)");
+    return B200Z_E_THROW;
+  }
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  std::vector<ZipAesMember> aes(n);
+  size_t extent = 0;
+  for (size_t k = 0; k < n; ++k) {
+    if (off[k] + len[k] < off[k]) return B200Z_E_ARG;
+    ZipAesMember &m = aes[k];
+    memset(&m, 0, sizeof m);
+    m.src_off = m.dst_off = off[k];
+    m.len = len[k];
+    m.salt_len = 16;
+    m.key_len = 32;
+    memcpy(m.salt, salts + 16 * k, 16);
+    extent = std::max(extent, (size_t)(off[k] + len[k]));
+  }
+  std::vector<ZipCtrTile> tiles;
+  ctr_tiles(aes, tiles);
+  const CryptLayout cl(n, tiles.size(), 0);
+  CU(g.d_crypt.reserve(cl.bytes));
+  CU(g.d_in.reserve(extent + 64));
+  uint8_t *dc = (uint8_t *)g.d_crypt.p, *d_base = (uint8_t *)g.d_in.p;
+  ZipHmacPads pads;
+  zip_hmac_pads(password, password_len, &pads);
+  if (extent) CU(cudaMemcpyAsync(d_base, data, extent, cudaMemcpyHostToDevice, g.stream));
+  CU(cudaMemsetAsync(d_base + extent, 0, 64, g.stream));
+  CU(cudaMemcpyAsync(dc + cl.members, aes.data(), n * sizeof(ZipAesMember), cudaMemcpyHostToDevice, g.stream));
+  CU(cudaMemcpyAsync(dc + cl.tiles, tiles.data(), tiles.size() * sizeof(ZipCtrTile), cudaMemcpyHostToDevice, g.stream));
+  const ZipAesMember *dm = (const ZipAesMember *)(dc + cl.members);
+  CU(zip_launch_pbkdf2(dm, (uint32_t)n, pads, dc + cl.dk, (uint32_t *)(dc + cl.rk), dc + cl.ver, g.stream));
+  CU(zip_launch_aes_ctr(dm, (const uint32_t *)(dc + cl.rk), (const ZipCtrTile *)(dc + cl.tiles), (uint32_t)tiles.size(), d_base,
+                        g.stream));
+  CU(zip_launch_hmac(dm, (uint32_t)n, dc + cl.dk, d_base, true, dc + cl.mac, g.stream));
+  if (extent) CU(cudaMemcpyAsync(data, d_base, extent, cudaMemcpyDeviceToHost, g.stream));
+  CU(cudaMemcpyAsync(pwd_verify, dc + cl.ver, 2 * n, cudaMemcpyDeviceToHost, g.stream));
+  CU(cudaMemcpyAsync(mac, dc + cl.mac, 10 * n, cudaMemcpyDeviceToHost, g.stream));
+  CU(cudaStreamSynchronize(g.stream));
+  return B200Z_OK;
+}
+
+// kernel times of the last b200z_zip_extract_password call (ms): PBKDF2, CTR, MAC (from the moment it may start), ZipCrypto
+extern "C" void b200z_debug_zip_crypt_ms(double out[4]) {
+  for (int k = 0; k < 4; ++k) out[k] = g_crypt_ms[k];
 }
 
 extern "C" {
@@ -2218,7 +2580,7 @@ void b200z_shutdown(void) {
   if (!g.inited) return;
   cudaSetDevice(g.device);
   cudaStreamSynchronize(g.stream);
-  g.d_in.release(); g.d_out.release(); g.d_ws.release(); g.d_meta.release(); g.d_small.release(); g.d_bz.release(); g.d_tok.release();
+  g.d_in.release(); g.d_out.release(); g.d_ws.release(); g.d_meta.release(); g.d_small.release(); g.d_bz.release(); g.d_tok.release(); g.d_crypt.release();
   g.h_meta.release();
   cudaStreamDestroy(g.stream);
   cudaStreamDestroy(g.s_h2d);

@@ -147,4 +147,36 @@ cudaError_t deflate_stored_device(const uint8_t *d_in, const DeflStoredBlock *h_
                                   size_t out_cap, void *ws, size_t ws_bytes, size_t *out_len, cudaStream_t s);
 cudaError_t crc32_tiles_device(const uint8_t *d_in, size_t n, uint32_t tile, uint32_t *d_part, cudaStream_t s);
 
+// ---- encrypted ZIP members (zip_crypt_kernels.cu) ----
+struct ZipAesMember {   // one WinZip AES member; offsets are bytes from the device base pointer of the call
+  uint64_t src_off;     // ciphertext (decrypt) / plaintext (encrypt)
+  uint64_t dst_off;     // where the CTR pass writes (may equal src_off)
+  uint64_t len;         // bytes of ciphertext
+  uint32_t salt_len;    // 8 / 12 / 16
+  uint32_t key_len;     // 16 / 24 / 32
+  uint8_t salt[16];
+};
+struct ZipCryptoMember {  // one ZipCrypto member: len bytes at src_off (12-byte header included) -> len - 12 at dst_off
+  uint64_t src_off, dst_off, len;
+};
+struct ZipCtrTile {  // one CTA of k_zip_aes_ctr: zip_ctr_tile_blocks() 16-byte blocks of one member from first_block on
+  uint64_t first_block;
+  uint32_t member, pad_;
+};
+struct ZipHmacPads {  // SHA-1 states after the HMAC inner / outer pad block of the password
+  uint32_t ipad[5], opad[5];
+};
+void zip_hmac_pads(const uint8_t *key, size_t klen, ZipHmacPads *p);
+void zipcrypto_keys(const uint8_t *pw, size_t len, uint32_t k[3]);  // the three keys after the password (host)
+uint64_t zip_ctr_tile_blocks();
+// d_dk: 80 bytes per member (derived key), d_rk: 60 words per member (AES round keys), d_ver: 2 bytes per member
+cudaError_t zip_launch_pbkdf2(const ZipAesMember *d_m, uint32_t n, const ZipHmacPads &pads, uint8_t *d_dk, uint32_t *d_rk,
+                              uint8_t *d_ver, cudaStream_t s);
+cudaError_t zip_launch_aes_ctr(const ZipAesMember *d_m, const uint32_t *d_rk, const ZipCtrTile *d_tiles, uint32_t n_tiles,
+                               uint8_t *d_base, cudaStream_t s);
+// 10 bytes of MAC per member over the bytes at src_off, or at dst_off when after_ctr (encryption: MAC of the ciphertext)
+cudaError_t zip_launch_hmac(const ZipAesMember *d_m, uint32_t n, const uint8_t *d_dk, const uint8_t *d_base, bool after_ctr,
+                            uint8_t *d_mac, cudaStream_t s);
+cudaError_t zip_launch_zipcrypto(const ZipCryptoMember *d_m, uint32_t n, const uint32_t keys[3], uint8_t *d_base, cudaStream_t s);
+
 }  // namespace b200z

@@ -80,8 +80,8 @@ def get_input_extension(input_path: str) -> str:
 _EXTENSIONS = ".tar.gz, .tgz, .tar.bz2, .tbz or .zip"
 
 
-def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | None = None) -> list:
-    """extractFileToDisk (:160-267).  .zip: ZipDecoder().decodeStream(InputFileStream) and the member loop above.
+def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | None = None, password=None) -> list:
+    """extractFileToDisk (:160-267).  .zip: ZipDecoder().decodeStream(InputFileStream, password:) and the member loop above.
     .tar.gz / .tgz / .tar.bz2 / .tbz: the reference decodes into a temporary `temp.tar` with
     GZipDecoder / BZip2Decoder.decodeStream(InputFileStream, OutputFileStream) (:183-202) and hands that to TarDecoder; here
     the same two stream objects make the library decode file -> file, and the .tar itself is the result (see the module
@@ -92,7 +92,7 @@ def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | N
     if ext == ".zip":
         inp = InputFileStream(input_path)
         try:
-            archive = ZipDecoder().decode_stream(inp)
+            archive = ZipDecoder().decode_stream(inp, password=password)
         finally:
             inp.close_sync()
         return extract_archive_to_disk(archive, output_path, buffer_size=buffer_size)

@@ -2,16 +2,36 @@
 `Archive` of `ArchiveFile`s, as lib/src/codecs/zip_decoder.dart:18-81 builds it.  The directory is parsed by
 b200z_zip_list (ZipDirectory / ZipFileHeader / ZipFile.read), and -- this is the point of the batching -- ALL members are
 decompressed by ONE b200z_zip_extract call (every deflate member is a unit of the same inflate batch) instead of one
-Inflate per member on first access (zip_file.dart:201-248)."""
+Inflate per member on first access (zip_file.dart:201-248).  With a password, ZipCrypto and WinZip AES members are
+decrypted on the device in the same call (b200z_zip_extract_password)."""
 from __future__ import annotations
 
 import ctypes as C
 
 from . import _ffi
 
-U_DONE, U_EOS, U_STOP, U_NOSPC = 0, 1, -1, -2
-ZIP_ENCRYPTED, ZIP_TOO_LARGE = -20, -21
+U_DONE, U_EOS, U_STOP, U_NOSPC, U_THROW = 0, 1, -1, -2, -5
+ZIP_ENCRYPTED, ZIP_TOO_LARGE, ZIP_BAD_PASSWORD, ZIP_BAD_MAC = -20, -21, -22, -23
+CRYPT_NONE, CRYPT_ZIPCRYPTO, CRYPT_AES = 0, 1, 2
 COMPRESSION = {0: "none", 8: "deflate", 12: "bzip2"}  # zip_file.dart:36-40; anything else is read as "none" (:83)
+
+
+class ArchiveException(Exception):
+    """util/archive_exception.dart: what the reference throws when an encrypted member cannot be read."""
+
+
+def password_bytes(password) -> bytes | None:
+    """The bytes the reference hashes / feeds the ZipCrypto keys: Dart's `codeUnits` (UTF-16 code units) cut to 8 bits
+    (zip_file.dart:264-266, 350).  Python strings iterate code points, so the string goes through UTF-16 first."""
+    if password is None:
+        return None
+    if isinstance(password, str):
+        return password.encode("utf-16-le")[::2]
+    return bytes(password)
+
+
+_CRYPT_ERRORS = {ZIP_BAD_PASSWORD: "password error", ZIP_BAD_MAC: "macs don't match",
+                 U_THROW: "encrypted member too short for its header, or an empty password (Dart: RangeError)"}
 
 
 def _name(raw: bytes) -> str:
@@ -33,12 +53,15 @@ class ArchiveFile:
         self.symbolic_link = None
         self.content = b"" if is_file else None
         self.status = U_DONE  # unit status of the member's decode (include/b200z.h)
+        self.encrypted = False  # decrypted with a password (the errors below are then the reference's throws)
 
     @property
     def is_symbolic_link(self):
         return bool(self.symbolic_link)
 
     def read_bytes(self):
+        if self.encrypted and self.status in _CRYPT_ERRORS:  # ZipFile.getStream throws on access (zip_file.dart:333-341)
+            raise ArchiveException(f"{self.name}: {_CRYPT_ERRORS[self.status]}")
         return self.content
 
 
@@ -100,10 +123,22 @@ class ZipDecoder:
             input.position = len(input.buffer)
         return self.decode_bytes(data, verify=verify, password=password)
 
+    def crypt_info(self, data, entry):
+        """-> (mode CRYPT_*, AES strength byte, method the content is stored with), as ZipFile.read decides
+        (b200z_zip_crypt_info); raises DartRangeError where the reference's extra-field scan throws."""
+        L = _ffi.lib()
+        addr, n, keep = _ffi.as_buffer(data)
+        mode, strength, method = C.c_uint32(), C.c_uint32(), C.c_uint32()
+        _ffi.check(L.b200z_zip_crypt_info(addr, n, C.byref(entry), C.byref(mode), C.byref(strength), C.byref(method)))
+        return mode.value, strength.value, method.value
+
     def decode_bytes(self, data, verify: bool = False, password=None) -> Archive:
+        """password: str (Dart's code units cut to 8 bits, see password_bytes) or bytes.  Without one, encrypted members
+        keep status ZIP_ENCRYPTED and empty content."""
         data = bytes(data) if not isinstance(data, (bytes, bytearray)) else data
+        pw = password_bytes(password)
         ents, n = self.list(data)
-        contents, statuses = self._extract(data, ents, n)
+        contents, statuses = self._extract(data, ents, n, pw)
         archive = Archive()
         for i in range(n):
             e = ents[i]
@@ -112,12 +147,22 @@ class ZipDecoder:
             entry = archive.find(name)
             if entry is None:
                 entry = ArchiveFile(name, 0, is_file=False) if is_dir else ArchiveFile(name, e.uncomp_size if e.has_data else 0)
-                entry.compression = COMPRESSION.get(e.method, "none") if e.has_data else "none"
+                method = e.method
+                if e.has_data and (e.flags & 1):  # an AES member names its real method in its extra record (:125-127)
+                    try:
+                        method = self.crypt_info(data, e)[2]
+                    except _ffi.B200ZError:
+                        pass
+                entry.compression = COMPRESSION.get(method, "none") if e.has_data else "none"
                 if not is_dir:
                     entry.content, entry.status = contents[i], statuses[i]
+                    entry.encrypted = pw is not None and bool(e.has_data and (e.flags & 1))
                 archive.add(entry)
             entry.mode = e.ext_attr >> 16
             if (e.version_made_by >> 8) == 3 and (entry.mode & 0xF000) == 0xA000:  # unix symlink (:58-70)
+                if pw is not None and e.has_data and (e.flags & 1) and statuses[i] in _CRYPT_ERRORS:
+                    # decodeStream reads a symlink's content while it walks the directory: the throw happens here
+                    raise ArchiveException(f"{name}: {_CRYPT_ERRORS[statuses[i]]}")
                 try:
                     entry.symbolic_link = contents[i].decode("utf-8")
                 except UnicodeDecodeError:
@@ -126,7 +171,7 @@ class ZipDecoder:
             entry.last_mod_time = (e.mod_date << 16) | e.mod_time
         return archive
 
-    def _extract(self, data, ents, n):
+    def _extract(self, data, ents, n, password=None):
         if n == 0:
             return [], []
         L = _ffi.ensure_init()
@@ -144,8 +189,9 @@ class ZipDecoder:
             out = (C.c_uint8 * max(tot, 1))()
             a64 = lambda l: (C.c_uint64 * m)(*l)
             out_len, st = (C.c_uint64 * m)(), (C.c_int32 * m)()
-            _ffi.check(L.b200z_zip_extract(addr, zlen, sub, m, C.addressof(out), max(tot, 1), a64(off),
-                                           a64([room[i] for i in todo]), out_len, st, self.flags))
+            _ffi.check(L.b200z_zip_extract_password(addr, zlen, sub, m, C.addressof(out), max(tot, 1), a64(off),
+                                                    a64([room[i] for i in todo]), out_len, st, self.flags, password,
+                                                    len(password or b"")))
             again = []
             for k, i in enumerate(todo):
                 statuses[i] = st[k]
@@ -222,20 +268,53 @@ def deflate_batch(contents, level: int = 6, window_bits: int = 15):
     return [(out[int(out_off[i]):int(out_off[i] + out_len[i])].tobytes(), int(crc[i])) for i in range(n)]
 
 
+def aes_encrypt_batch(payloads, salts, password: bytes):
+    """ZipEncoder._encryptCompressedData (zip_encoder.dart:166-183) for every payload at once: ONE b200z_zip_aes_encrypt call
+    (key derivation, AES-256-CTR and the MAC on the device) -> list of (ciphertext, verifier, mac)."""
+    import numpy as np
+    L = _ffi.ensure_init()
+    n = len(payloads)
+    if n == 0:
+        return []
+    ln = np.array([len(p) for p in payloads], dtype=np.uint64)
+    off = np.zeros(n, dtype=np.uint64)
+    off[1:] = np.cumsum(ln)[:-1]
+    buf = bytearray(b"".join(bytes(p) for p in payloads) or b"\0")
+    addr, nb, keep = _ffi.as_buffer(buf)
+    salt = b"".join(salts)
+    assert len(salt) == 16 * n
+    ver, mac = (C.c_uint8 * (2 * n))(), (C.c_uint8 * (10 * n))()
+    _ffi.check(L.b200z_zip_aes_encrypt(addr, off.ctypes.data, ln.ctypes.data, n, salt, password, len(password), ver, mac))
+    data = bytes(keep)
+    return [(data[int(off[i]):int(off[i] + ln[i])], bytes(ver[2 * i:2 * i + 2]), bytes(mac[10 * i:10 * i + 10])) for i in range(n)]
+
+
 class ZipEncoder:
     """`ZipEncoder().encode_bytes(archive, level: 1, modified:)` (zip_encoder.dart:66-121): local headers + data, central
     directory, (zip64) end records, written field by field as `_writeFile` :309-372 and `_writeCentralDirectory` :391-497 do.
     Members are compressed on the device (`compress` exists so that the CPU test tier can check the container logic with a
     stand-in).  Not mirrored: encryption, and passing already-compressed members through (`file.isCompressed`, :214-235) --
-    the ArchiveFile of this package holds content, not the source archive's bytes."""
+    the ArchiveFile of this package holds content, not the source archive's bytes.
+
+    With `password` (ZipEncoder(password:), :166-183, 270-310, 347-437) every member is AES-256 encrypted as the reference
+    writes it: all payloads go through ONE b200z_zip_aes_encrypt call, and the container keeps the reference's quirks --
+    method 99, flag bit 0 and an AE-1 record on every entry, directories included; the verifier and MAC of the last
+    encrypted member stay with the encoder, so a directory after a file gets compressedSize 12 and that file's MAC (10 bytes)
+    behind its local header."""
 
     VERSION = 20
 
-    def __init__(self, compress=None, batch: bool = False):
+    def __init__(self, compress=None, batch: bool = False, password=None, salt=None, encrypt=None):
         """batch=True: all deflate members go to the device in one b200z_deflate_batch call (several members in flight)
-        instead of one b200z_deflate_raw call each; the archive bytes are the same."""
+        instead of one b200z_deflate_raw call each; the archive bytes are the same.  password: str or bytes (see
+        password_bytes); salt: callable returning each member's 16 salt bytes (default os.urandom, as Random.secure);
+        encrypt: stand-in for aes_encrypt_batch (the CPU test tier)."""
+        import os
         self._compress = compress or _b200_compress
         self._batch = batch and compress is None
+        self._password = password_bytes(password)
+        self._salt = salt or (lambda: os.urandom(16))
+        self._encrypt = encrypt or aes_encrypt_batch
 
     def encode_bytes(self, archive, level: int = 1, modified=None, comment: str = "") -> bytes:
         import struct
@@ -258,18 +337,38 @@ class ZipEncoder:
 
             def compress(content, method, level_):
                 return table[at[0]] if method == "deflate" else self._compress(content, method, level_)
+        pw = self._password
+        payloads = []
         for pos_in_archive, entry in enumerate(archive):
             if self._batch:
                 at[0] = pos_in_archive
+            method = (entry.compression or "deflate") if entry.is_file else "deflate"
+            payloads.append(compress(entry.content or b"", method, level_of(entry)) if entry.is_file else None)
+        sealed = {}
+        if pw is not None:  # _encryptCompressedData for every file, in one device call
+            if not pw:
+                raise _ffi.DartRangeError(_ffi.E_THROW, "ZipEncoder: empty password (ZipFile.deriveKey returns an empty list)")
+            idx = [i for i, p in enumerate(payloads) if p is not None]
+            salts = {i: bytes(self._salt()) for i in idx}
+            sealed = dict(zip(idx, ((salts[i],) + r for i, r in zip(idx, self._encrypt([payloads[i][0] for i in idx],
+                                                                                      [salts[i] for i in idx], pw)))))
+        last_ver = last_mac = None  # _pwdVer / _mac: fields of the encoder, they outlive the member they belong to
+        for pos_in_archive, entry in enumerate(archive):
             lm = time.localtime(modified if modified is not None else entry.last_mod_time)  # DateTime.fromMillisecondsSinceEpoch
             name = entry.name.replace("\\", "/")
             if not entry.is_file and not name.endswith("/"):
                 name += "/"
             method = (entry.compression or "deflate") if entry.is_file else "deflate"
-            payload, crc = b"", 0
-            if entry.is_file:
-                payload, crc = compress(entry.content or b"", method, level_of(entry))
-            fd = dict(name=name, time=_dos_time(lm), date=_dos_date(lm), crc=crc, csize=len(payload),
+            payload, crc = payloads[pos_in_archive] or (b"", 0)
+            head = tail = b""
+            if pos_in_archive in sealed:
+                salt, payload, last_ver, last_mac = sealed[pos_in_archive]
+                head = salt + last_ver
+            if pw is not None and last_mac is not None:
+                tail = last_mac
+            # dataLen (:283-286): data + salt (files only) + the encoder's current MAC and verifier, whoever they belong to
+            csize = len(payload) + (16 if pos_in_archive in sealed else 0) + (12 if tail else 0)
+            fd = dict(name=name, time=_dos_time(lm), date=_dos_date(lm), crc=crc, csize=csize,
                       usize=entry.size if entry.is_file else 0, method=method, mode=entry.mode, pos=len(out),
                       comment=getattr(entry, "comment", None) or "")
             files.append(fd)
@@ -277,10 +376,13 @@ class ZipEncoder:
             z64 = fd["csize"] > 0xFFFFFFFF or fd["usize"] > 0xFFFFFFFF
             extra = struct.pack("<BBBBQQ", 1, 0, 0x10, 0, fd["usize"], fd["csize"]) if z64 else b""
             m = {"deflate": 8, "bzip2": 12}.get(method, 0)
+            if pw is not None:
+                extra += self._aes_extra(m)
             nb = name.encode("utf-8")
-            out += struct.pack("<IHHHHHIIIHH", 0x04034B50, self.VERSION, 0x800, m, fd["time"], fd["date"], crc,
+            out += struct.pack("<IHHHHHIIIHH", 0x04034B50, self.VERSION, 0x801 if pw is not None else 0x800,
+                               99 if pw is not None else m, fd["time"], fd["date"], crc,
                                0xFFFFFFFF if z64 else fd["csize"], 0xFFFFFFFF if z64 else fd["usize"], len(nb), len(extra))
-            out += nb + extra + payload
+            out += nb + extra + head + payload + tail
         # _writeCentralDirectory
         cd_pos = len(out)
         any64 = False
@@ -289,8 +391,11 @@ class ZipEncoder:
             any64 |= z64
             extra = struct.pack("<BBBBQQQ", 1, 0, 0x18, 0, fd["usize"], fd["csize"], fd["pos"]) if z64 else b""
             m = {"deflate": 8, "bzip2": 12}.get(fd["method"], 0)
+            if pw is not None:
+                extra += self._aes_extra(m)
             nb, cb = fd["name"].encode("utf-8"), fd["comment"].encode("utf-8")
-            out += struct.pack("<IHHHHHHIIIHHHHHII", 0x02014B50, (0 << 8) | self.VERSION, self.VERSION, 0x800, m, fd["time"],
+            out += struct.pack("<IHHHHHHIIIHHHHHII", 0x02014B50, (0 << 8) | self.VERSION, self.VERSION,
+                               0x801 if pw is not None else 0x800, 99 if pw is not None else m, fd["time"],
                                fd["date"], fd["crc"], 0xFFFFFFFF if z64 else fd["csize"], 0xFFFFFFFF if z64 else fd["usize"],
                                len(nb), len(extra), len(cb), 0, 0, (fd["mode"] << 16) & 0xFFFFFFFF,
                                0xFFFFFFFF if z64 else fd["pos"])
@@ -307,5 +412,10 @@ class ZipEncoder:
                            0xFFFF if need64 else n, 0xFFFFFFFF if need64 else cd_size, 0xFFFFFFFF if need64 else cd_pos, len(cb))
         out += cb
         return bytes(out)
+
+    @staticmethod
+    def _aes_extra(method_id: int) -> bytes:  # _getAexExtraData :347-363: AE-1, vendor "AE", strength 3 (256 bits)
+        import struct
+        return struct.pack("<HHH2sBH", 0x9901, 7, 1, b"AE", 3, method_id)
 
     encode = encode_bytes

@@ -114,6 +114,20 @@ typedef _ZipExtractC = Int32 Function(Pointer<Uint8> zip, Size zipLen, Pointer<Z
     Size outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen, Pointer<Int32> status, Uint32 flags);
 typedef _ZipExtractD = int Function(Pointer<Uint8> zip, int zipLen, Pointer<ZipEntry> entries, int n, Pointer<Uint8> out,
     int outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen, Pointer<Int32> status, int flags);
+typedef _ZipCryptInfoC = Int32 Function(Pointer<Uint8> zip, Size zipLen, Pointer<ZipEntry> entry, Pointer<Uint32> mode,
+    Pointer<Uint32> aesStrength, Pointer<Uint32> method);
+typedef _ZipCryptInfoD = int Function(Pointer<Uint8> zip, int zipLen, Pointer<ZipEntry> entry, Pointer<Uint32> mode,
+    Pointer<Uint32> aesStrength, Pointer<Uint32> method);
+typedef _ZipExtractPasswordC = Int32 Function(Pointer<Uint8> zip, Size zipLen, Pointer<ZipEntry> entries, Size n,
+    Pointer<Uint8> out, Size outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen,
+    Pointer<Int32> status, Uint32 flags, Pointer<Uint8> password, Size passwordLen);
+typedef _ZipExtractPasswordD = int Function(Pointer<Uint8> zip, int zipLen, Pointer<ZipEntry> entries, int n,
+    Pointer<Uint8> out, int outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen,
+    Pointer<Int32> status, int flags, Pointer<Uint8> password, int passwordLen);
+typedef _ZipAesEncryptC = Int32 Function(Pointer<Uint8> data, Pointer<Uint64> off, Pointer<Uint64> len, Size n,
+    Pointer<Uint8> salts, Pointer<Uint8> password, Size passwordLen, Pointer<Uint8> pwdVerify, Pointer<Uint8> mac);
+typedef _ZipAesEncryptD = int Function(Pointer<Uint8> data, Pointer<Uint64> off, Pointer<Uint64> len, int n,
+    Pointer<Uint8> salts, Pointer<Uint8> password, int passwordLen, Pointer<Uint8> pwdVerify, Pointer<Uint8> mac);
 
 
 // ---- the rest of include/b200z.h: batches, sharding, checksums, diagnostics ----
@@ -221,6 +235,10 @@ class B200Z {
   late final _ZipListD zipList = _lib.lookupFunction<_ZipListC, _ZipListD>('b200z_zip_list');
   late final _ZipExtractD zipExtract = _lib.lookupFunction<_ZipExtractC, _ZipExtractD>('b200z_zip_extract');
   late final _ZipCommentD zipComment = _lib.lookupFunction<_ZipCommentC, _ZipCommentD>('b200z_zip_comment');
+  late final _ZipCryptInfoD zipCryptInfo = _lib.lookupFunction<_ZipCryptInfoC, _ZipCryptInfoD>('b200z_zip_crypt_info');
+  late final _ZipExtractPasswordD zipExtractPassword =
+      _lib.lookupFunction<_ZipExtractPasswordC, _ZipExtractPasswordD>('b200z_zip_extract_password');
+  late final _ZipAesEncryptD zipAesEncrypt = _lib.lookupFunction<_ZipAesEncryptC, _ZipAesEncryptD>('b200z_zip_aes_encrypt');
   late final _Bz2ShardD bzip2DecodeShard = _lib.lookupFunction<_Bz2ShardC, _Bz2ShardD>('b200z_bzip2_decode_shard');
   late final _Crc32D crc32 = _lib.lookupFunction<_Crc32C, _Crc32D>('b200z_crc32');
   late final _DeflateBatchD deflateBatch = _lib.lookupFunction<_DeflateBatchC, _DeflateBatchD>('b200z_deflate_batch');

@@ -280,7 +280,8 @@ class BZip2Encoder {
   }
 }
 
-/// ZipDecoder (zip_decoder.dart:18-81) with all members decompressed by ONE b200z_zip_extract call.
+/// ZipDecoder (zip_decoder.dart:18-81) with all members decompressed by ONE b200z_zip_extract_password call; the password
+/// (if any) goes to the library as the low bytes of its code units, as ZipFile.deriveKey / _initKeys use it.
 class ZipDecoder {
   ar.Archive decodeBytes(List<int> bytes, {bool verify = false, String? password}) {
     final z = B200Z.instance;
@@ -307,8 +308,12 @@ class ZipDecoder {
           total += (r + 63) & ~63;
         }
         final out = z.hostAlloc(total == 0 ? 64 : total);
+        final pw = password == null ? nullptr : calloc<Uint8>(password.length + 1);
+        for (var i = 0; password != null && i < password.length; i++) {
+          pw[i] = password.codeUnitAt(i) & 0xff;
+        }
         try {
-          rc = z.zipExtract(inp, bytes.length, ents, count, out, total, off, room, len, st, 0);
+          rc = z.zipExtractPassword(inp, bytes.length, ents, count, out, total, off, room, len, st, 0, pw, password?.length ?? 0);
           if (rc != b200zOk) throw B200ZException(rc, z.lastError);
           // (members whose size fields lied report B200Z_U_NOSPC: retry those with more room, as archive_b200/zip.py does)
           final all = out.asTypedList(total == 0 ? 0 : total);
@@ -317,6 +322,10 @@ class ZipDecoder {
             final name = e.hasData != 0 ? String.fromCharCodes(bytes.sublist(e.nameOff, e.nameOff + e.nameLen)) : '';
             if (archive.find(name) != null) continue;
             final isDir = name.endsWith('/') || name.endsWith('\\');
+            // the reference throws when such a member is read (zip_file.dart:333-341); this shim reads every member here
+            if (st[i] == -22) throw Exception('password error');
+            if (st[i] == -23) throw Exception('macs don\'t match');
+            if (st[i] == -5) throw RangeError('$name: encrypted member too short, or an empty password');
             final content = Uint8List.fromList(all.sublist(off[i], off[i] + (len[i] < room[i] ? len[i] : room[i])));
             final f = isDir ? ar.ArchiveFile.directory(name) : ar.ArchiveFile.bytes(name, content);
             f.mode = e.extAttr >> 16;
@@ -326,6 +335,7 @@ class ZipDecoder {
           }
         } finally {
           z.hostFree(out);
+          if (pw != nullptr) calloc.free(pw);
         }
         return archive;
       } finally {

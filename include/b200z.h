@@ -151,7 +151,8 @@ int b200z_crc32(const uint8_t *in, size_t in_len, uint32_t *crc);
  * b200z_zip_extract = ZipFile.getStream / decompress (zip_file.dart:164-249) for ALL listed members at once: the deflate
  *                    members are one batch of the inflate kernels, stored members are copies, bzip2 members are
  *                    decoded one after the other.  Names are byte ranges of the archive (decoding them is the host
- *                    language's business).  Encrypted members (ZipCrypto / AES) are reported, not decoded.        */
+ *                    language's business).  Encrypted members (ZipCrypto / AES) are reported, not decoded, unless a
+ *                    password is given (b200z_zip_extract_password).                                                    */
 typedef struct {
   uint64_t local_header_off; /* ZipFileHeader.localHeaderOffset (zip64 applied)                               */
   uint64_t data_off;         /* first byte of the member's data; valid when has_data                          */
@@ -176,6 +177,35 @@ int b200z_zip_comment(const uint8_t *zip, size_t zip_len, uint64_t *off, uint32_
 int b200z_zip_extract(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                       size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
                       int32_t *status, uint32_t flags);
+/* Encrypted members -- ZipDecoder().decodeBytes(bytes, password:) (zip_file.dart:98-134, 164-216, 260-359).
+ * b200z_zip_crypt_info (host only): how member `e` is encrypted, as ZipFile.read decides it: flag bit 0 is ZipCrypto unless
+ * the LOCAL extra field (longer than 2 bytes) holds an AES record (id 0x9901); `method` is the method the content is stored
+ * with (the AES record's for AES members), `aes_strength` the record's strength byte (1: 128, 2: 192, else 256 bits).  The
+ * reference's scan walks the extra field in 2-byte steps without skipping other records' payloads; when that walk reads
+ * past the end (ZipFile.read throws): B200Z_E_THROW.
+ * b200z_zip_extract_password: b200z_zip_extract with a password (`password_len` bytes: the low byte of each UTF-16 code
+ * unit, as the reference's codeUnits; length 0 is the empty password).  password == NULL is exactly b200z_zip_extract.
+ * Per member, beyond the B200Z_U_* statuses: B200Z_ZIP_BAD_PASSWORD (AES verifier mismatch), B200Z_ZIP_BAD_MAC (the
+ * HMAC-SHA1 of the ciphertext does not match; the member was decoded, its bytes are withheld), B200Z_U_THROW (the member
+ * is too short for its ZipCrypto header / AES salt + verifier + MAC, an empty password on an AES member, or the extra field
+ * scan throws); out_len = 0 for all three.  ZipCrypto has no check: a wrong password decodes to garbage, as in the
+ * reference.  The reference decrypts inside the caller's archive buffer; `zip` is const here and stays as it was.     */
+#define B200Z_ZIP_CRYPT_NONE 0u
+#define B200Z_ZIP_CRYPT_ZIPCRYPTO 1u
+#define B200Z_ZIP_CRYPT_AES 2u
+#define B200Z_ZIP_BAD_PASSWORD (-22) /* status: AES password verifier mismatch (Exception('password error'))       */
+#define B200Z_ZIP_BAD_MAC (-23)      /* status: AES authentication code mismatch                                 */
+int b200z_zip_crypt_info(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *e, uint32_t *mode,
+                         uint32_t *aes_strength, uint32_t *method);
+int b200z_zip_extract_password(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
+                               size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
+                               int32_t *status, uint32_t flags, const uint8_t *password, size_t password_len);
+/* ZipEncoder(password:) member payloads (zip_encoder.dart:166-183): AES-256 in place on host buffers.  Member i is
+ * data[off[i] .. +len[i]) (already compressed), salts[16 i ..] its salt; on return it is the ciphertext,
+ * pwd_verify[2 i ..] its password verifier and mac[10 i ..] the first 10 bytes of the HMAC-SHA1 of the ciphertext.  An
+ * empty password: B200Z_E_THROW (the reference's deriveKey returns an empty list and sublist throws).               */
+int b200z_zip_aes_encrypt(uint8_t *data, const uint64_t *off, const uint64_t *len, size_t n, const uint8_t *salts,
+                          const uint8_t *password, size_t password_len, uint8_t *pwd_verify, uint8_t *mac);
 
 /* ---- file streams: InputFileStream -> codec -> OutputFileStream -------------------------------------------------
  * decodeStream / encodeStream with an InputFileStream and an OutputFileStream (input_file_stream.dart:11-221,

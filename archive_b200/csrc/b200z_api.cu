@@ -2616,7 +2616,7 @@ int b200z_inflate_batch_device(const uint8_t *d_in_base, const uint64_t *d_in_of
   if (rc) return rc;
   if (n_units == 0) return B200Z_OK;
   const size_t extent = inflate_ws_extent_for(n_units, workspace_bytes_);
-  if (extent == 0) {
+  if (extent == INFLATE_WS_TOO_SMALL) {
     set_err("inflate_batch_device: workspace too small (size it with b200z_inflate_workspace_bytes)");
     return B200Z_E_ARG;
   }

@@ -34,7 +34,9 @@ struct InflateWs {
   uint32_t hist = 0;
 };
 size_t inflate_ws_bytes(size_t n_units, size_t extent);
-size_t inflate_ws_extent_for(size_t n_units, size_t bytes);  // largest extent a workspace of `bytes` serves
+// largest extent a workspace of `bytes` serves (extent 0 is valid); INFLATE_WS_TOO_SMALL when it serves none
+constexpr size_t INFLATE_WS_TOO_SMALL = ~(size_t)0;
+size_t inflate_ws_extent_for(size_t n_units, size_t bytes);
 InflateWs inflate_ws_carve(void *ws, size_t n_units, size_t extent);
 InflateWs inflate_ws_slice(const InflateWs &w, size_t first_unit, size_t first_out_byte);
 

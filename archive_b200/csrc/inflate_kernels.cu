@@ -349,10 +349,17 @@ size_t inflate_ws_bytes(size_t n_units, size_t extent) {
   const size_t ub = (n_units * (size_t)USCRATCH_BYTES + 255) & ~(size_t)255;
   return tok + hb + pb + ub + 256;
 }
+// The inverse of inflate_ws_bytes: the largest extent e with inflate_ws_bytes(n_units, e) <= bytes, so that a workspace
+// sized for extent E always serves at least E (its token region then covers every output byte of the layout).  Each
+// output byte costs 4 token bytes and about 4 * (SPEC_MAX_G - 1) / 2^SPEC_HSHIFT helper bytes; the estimate from that is
+// within a few hundred bytes' rounding of the answer, and the steps from it find the exact value.
 size_t inflate_ws_extent_for(size_t n_units, size_t bytes) {
-  const size_t fixed = inflate_ws_bytes(n_units, 0) + 1024;
-  if (bytes <= fixed) return 0;
-  return (bytes - fixed) / (4 + (SPEC_MAX_G - 1)) ;
+  const size_t fixed = inflate_ws_bytes(n_units, 0);
+  if (bytes < fixed) return INFLATE_WS_TOO_SMALL;
+  size_t e = (bytes - fixed) / (4 + ((4 * (SPEC_MAX_G - 1)) >> SPEC_HSHIFT));
+  while (e > 0 && inflate_ws_bytes(n_units, e) > bytes) --e;
+  while (inflate_ws_bytes(n_units, e + 1) <= bytes) ++e;
+  return e;
 }
 InflateWs inflate_ws_carve(void *ws, size_t n_units, size_t extent) {
   InflateWs w;

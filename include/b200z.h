@@ -248,8 +248,19 @@ int b200z_inflate_batch(const uint8_t *in_base, size_t in_bytes, const uint64_t 
                         const uint64_t *out_off, const uint32_t *out_cap, uint32_t *out_len,
                         int32_t *status, uint32_t *in_used, size_t n_units);
 /* Device-pointer variant: every pointer is device memory on the b200z_init device; work is
- * enqueued on `cuda_stream` (a cudaStream_t, NULL = the library's stream) and NOT synchronised.
- * `workspace` must hold b200z_inflate_workspace_bytes(...) bytes.                           */
+ * enqueued on `cuda_stream` (a cudaStream_t, NULL = the library's stream) and NOT synchronised:
+ * read the results after that stream has been synchronised.
+ * Input: d_in_base is 16-byte aligned, and the kernels read whole aligned 16-byte blocks, so
+ * the buffer must be readable through round_up(max(in_off[u] + in_len[u]), 16) bytes from
+ * d_in_base (what lies past a unit's in_len is read but never decoded).
+ * Output: unit u writes d_out_base[out_off[u] .. +out_cap[u]); slots may come in any order and
+ * leave gaps, which are not written.
+ * Workspace: `workspace` must hold b200z_inflate_workspace_bytes(n_units, total_in_bytes,
+ * total_out_cap) bytes, where total_out_cap is the layout's EXTENT, max(out_off[u] + out_cap[u])
+ * (not the sum of the caps: the workspace is indexed by out_off).  total_in_bytes is not used.
+ * The workspace needs no initialisation, may be reused by the next call on the same stream,
+ * and must not be shared by batches in flight at the same time.  A workspace smaller than
+ * b200z_inflate_workspace_bytes(n_units, 0, 0) gives B200Z_E_ARG with nothing enqueued.     */
 size_t b200z_inflate_workspace_bytes(size_t n_units, size_t total_in_bytes, size_t total_out_cap);
 int b200z_inflate_batch_device(const uint8_t *d_in_base, const uint64_t *d_in_off,
                                const uint32_t *d_in_len, uint8_t *d_out_base,

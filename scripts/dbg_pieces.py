@@ -26,7 +26,9 @@ PW, US = 2 + 3 * 30, 7 * 64 * 4
 def ws_b(nu, ext):
     tok = (ext * 4 + 511) & ~255; hs = (ext >> 2) + 64; hb = (7 * hs * 4 + 255) & ~255
     return tok + hb + ((nu * PW * 4 + 255) & ~255) + ((nu * US + 255) & ~255) + 256
-ext = (ws_bytes - (ws_b(n, 0) + 1024)) // 11
+ext = n * UNIT  # the largest extent with ws_b(n, ext) <= ws_bytes
+while ws_b(n, ext + 1) <= ws_bytes:
+    ext += 1
 tok = (ext * 4 + 511) & ~255; hs = (ext >> 2) + 64; hb = (7 * hs * 4 + 255) & ~255
 P = d_ws[tok + hb: tok + hb + n * PW * 4].cpu().numpy().view(np.uint32).reshape(n, PW)
 npc = P[:, 0]

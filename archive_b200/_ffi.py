@@ -16,6 +16,7 @@ LIB_PATH = os.environ.get("B200Z_LIB") or os.path.join(_HERE, "libb200z.so")
 
 OK, E_NODEVICE, E_ARG, E_NOSPC, E_DATA, E_THROW, E_INTERNAL = 0, -1, -2, -3, -4, -5, -6
 FILE_GZIP_DECODE, FILE_ZLIB_DECODE, FILE_BZIP2_DECODE, FILE_ZLIB_ENCODE, FILE_GZIP_ENCODE, FILE_BZIP2_ENCODE = 1, 2, 3, 4, 5, 6
+FILE_XZ_DECODE, FILE_XZ_ENCODE = 7, 8
 U_DONE, U_EOS, U_STOP, U_NOSPC, U_RANGE, U_BADCODE, U_THROW, U_TOKCAP = 0, 1, -1, -2, -3, -4, -5, -6
 
 
@@ -76,6 +77,11 @@ _SIGS = {
                                     C.POINTER(C.c_size_t)]),
     "b200z_bzip2_decode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_crc32": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]),
+    "b200z_xz_decode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "b200z_xz_bound": (C.c_size_t, [C.c_void_p, C.c_size_t]),
+    "b200z_xz_encode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "b200z_xz_encode_bound": (C.c_size_t, [C.c_size_t]),
+    "b200z_crc64": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]),
     "b200z_zip_list": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_zip_comment": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     "b200z_zip_extract": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,

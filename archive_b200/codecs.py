@@ -6,6 +6,7 @@ Mirrors (paths relative to /root/reference/):
   ZLibDecoder(Web)   lib/src/codecs/zlib_decoder.dart:14-35, codecs/zlib/_zlib_decoder_web.dart:14-107
   GZipDecoder(Web)   lib/src/codecs/gzip_decoder.dart:14-30, codecs/zlib/_gzip_decoder_web.dart:14-58
   inflateBuffer      lib/src/codecs/zlib/inflate_buffer.dart:7
+  XZDecoder / XZEncoder  lib/src/codecs/xz_decoder.dart, xz_encoder.dart; getCrc64 lib/src/util/crc64.dart
 
 In the Dart package these classes stay Dart and bind libb200z.so with dart:ffi (dart/, INTEGRATION.md);
 no Dart SDK exists in the build image, so the parity tests drive this Python mirror instead.
@@ -225,6 +226,75 @@ class BZip2Encoder:
         output.write_bytes(C.string_at(out, out_len.value))
         _consume(input)
         return True
+
+
+class XZCheck:
+    """XZCheck (lib/src/codecs/xz_encoder.dart:11): the values are the enum's indices."""
+    none, crc32, crc64, sha256 = 0, 1, 2, 3
+
+
+class XZDecoder:
+    """XZDecoder().decodeBytes / decodeStream (lib/src/codecs/xz_decoder.dart:15-27): one stream; block CRC-32 / CRC-64
+    checks are compared only when `verify`; decodeStream returns False on a container or check error and keeps what was
+    written before it; a Dart throw raises DartRangeError."""
+
+    def decode_bytes(self, data, verify: bool = False) -> bytes:
+        out = OutputMemoryStream()
+        self.decode_stream(InputMemoryStream(data), out, verify=verify)
+        return out.get_bytes()
+
+    def decode_stream(self, input: InputMemoryStream, output: OutputMemoryStream, verify: bool = False) -> bool:
+        if _both_files(input, output):
+            return _stream_result(_file_codec(_ffi.FILE_XZ_DECODE, input, output, int(verify)))
+        L = _ffi.ensure_init()
+        view = _rest(input)
+        addr, n, keep = _ffi.as_buffer(view)
+        out_len = C.c_size_t(0)
+
+        def call(oa, cap):
+            rc = L.b200z_xz_decode(addr, n, int(verify), oa, cap, C.byref(out_len))
+            return rc, out_len.value
+
+        rc, out, got = _grow_call(call, addr, n, L.b200z_xz_bound(addr, n) + 64)
+        if got and rc != _ffi.E_THROW:
+            output.write_bytes(C.string_at(out, got))
+        _consume(input)
+        return _stream_result(rc)
+
+
+class XZEncoder:
+    """XZEncoder().encodeBytes / encode / encodeStream (lib/src/codecs/xz_encoder.dart:18-62): one stored LZMA2 chunk
+    (its 16-bit length field is cut for inputs over 64 KiB, as in the reference) and the check, computed on the device."""
+
+    def encode_bytes(self, data, check: int = XZCheck.crc64) -> bytes:
+        out = OutputMemoryStream()
+        self.encode_stream(InputMemoryStream(data), out, check=check)
+        return out.get_bytes()
+
+    encode = encode_bytes
+
+    def encode_stream(self, input: InputMemoryStream, output: OutputMemoryStream, check: int = XZCheck.crc64):
+        if _both_files(input, output):
+            _ffi.check(_file_codec(_ffi.FILE_XZ_ENCODE, input, output, int(check)))
+            return
+        L = _ffi.ensure_init()
+        view = _rest(input)
+        addr, n, keep = _ffi.as_buffer(view)
+        cap = L.b200z_xz_encode_bound(n)
+        out = (C.c_uint8 * cap)()
+        out_len = C.c_size_t(0)
+        _ffi.check(L.b200z_xz_encode(addr, n, int(check), C.addressof(out), cap, C.byref(out_len)))
+        output.write_bytes(C.string_at(out, out_len.value))
+        _consume(input)
+
+
+def get_crc64(data) -> int:
+    """getCrc64 (lib/src/util/crc64.dart, _crc64_io.dart:5-11): ECMA-182 CRC-64, computed on the device."""
+    L = _ffi.ensure_init()
+    addr, n, keep = _ffi.as_buffer(data)
+    crc = C.c_uint64(0)
+    _ffi.check(L.b200z_crc64(addr, n, C.byref(crc)))
+    return crc.value
 
 
 class Deflate:

@@ -21,8 +21,9 @@
 #include "bzip2_enc.h"
 #ifdef B200Z_EMU
 // The CPU emulation build of the library compiles the generated copies of the .cu files it lists; the encrypted-member
-// kernels come in here (zip_crypt_kernels.cu launches through ZC_LAUNCH, which both compilers take).
+// and XZ kernels come in here (zip_crypt_kernels.cu and xz_kernels.cu launch through macros both compilers take).
 #include "zip_crypt_kernels.cu"
+#include "xz_kernels.cu"
 #endif
 
 namespace b200z {
@@ -1403,7 +1404,7 @@ static uint32_t crc_xpow8(uint64_t nbytes) {
 }
 static const uint32_t kCrcTile = 1u << 13;
 // CRC-32 of d[0, n) on stream s: tile CRCs into d_part ((n / kCrcTile + 1) words of device memory), folded on the host
-static int device_crc32_on(const uint8_t *d, size_t n, uint32_t *d_part, cudaStream_t s, uint32_t *out) {
+int device_crc32_on(const uint8_t *d, size_t n, uint32_t *d_part, cudaStream_t s, uint32_t *out) {
   const uint32_t TILE = kCrcTile;
   if (n == 0) {
     *out = 0;
@@ -2479,6 +2480,39 @@ int b200z_crc32(const uint8_t *in, size_t in_len, uint32_t *crc) {
   if (rc) return rc;
   return device_crc32((const uint8_t *)g.d_in.p, in_len, crc);
 }
+
+int b200z_xz_decode(const uint8_t *in, size_t in_len, int verify, uint8_t *out, size_t out_cap, size_t *out_len) {
+  int rc = require_init();
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  size_t n = 0;
+  rc = xz_decode_impl(in, in_len, verify, out, out_cap, &n, g.stream);
+  if (out_len) *out_len = n;
+  return rc;
+}
+size_t b200z_xz_bound(const uint8_t *in, size_t in_len) { return xz_bound(in, in_len); }
+int b200z_xz_encode(const uint8_t *in, size_t in_len, int check, uint8_t *out, size_t out_cap, size_t *out_len) {
+  int rc = require_init();
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  size_t n = 0;
+  rc = xz_encode_impl(in, in_len, check, out, out_cap, &n, g.stream);
+  if (out_len) *out_len = n;
+  return rc;
+}
+size_t b200z_xz_encode_bound(size_t in_len) { return xz_encode_bound(in_len); }
+int b200z_crc64(const uint8_t *in, size_t in_len, uint64_t *crc) {
+  int rc = require_init();
+  if (rc) return rc;
+  if (!crc) return B200Z_E_ARG;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return xz_crc64_impl(in, in_len, crc, g.stream);
+}
+// (debug, not part of the ABI) k_xz_lzma time in ms and the run count of the last b200z_xz_decode
+void b200z_debug_xz(double *lzma_ms, uint32_t *n_runs) { xz_debug(lzma_ms, n_runs); }
 
 int b200z_bzip2_decode_shard(const uint8_t *in, size_t in_len, uint32_t rank, uint32_t world, uint8_t *out, size_t out_cap,
                              size_t *out_len, b200z_bz2_block *blocks, size_t blocks_cap, size_t *n_blocks) {

@@ -144,6 +144,8 @@ size_t first_cap(const Args &a, const uint8_t *in, size_t n) {
     case B200Z_FILE_ZLIB_ENCODE:
     case B200Z_FILE_GZIP_ENCODE: return b200z_deflate_bound(n);
     case B200Z_FILE_BZIP2_ENCODE: return b200z_bzip2_bound(n);
+    case B200Z_FILE_XZ_DECODE: return b200z_xz_bound(in, n) + 64;
+    case B200Z_FILE_XZ_ENCODE: return b200z_xz_encode_bound(n);
   }
   return 0;
 }
@@ -161,6 +163,8 @@ int call_codec(const Args &a, const uint8_t *in, size_t n, uint8_t *out, size_t 
     case B200Z_FILE_ZLIB_ENCODE: return b200z_zlib_encode(in, n, a.a0, a.a1, (int)a.a2, out, cap, got);
     case B200Z_FILE_GZIP_ENCODE: return b200z_gzip_encode(in, n, a.a0, a.a2, out, cap, got);
     case B200Z_FILE_BZIP2_ENCODE: return b200z_bzip2_encode(in, n, out, cap, got);
+    case B200Z_FILE_XZ_DECODE: return b200z_xz_decode(in, n, a.a0, out, cap, got);
+    case B200Z_FILE_XZ_ENCODE: return b200z_xz_encode(in, n, a.a0, out, cap, got);
   }
   return B200Z_E_ARG;
 }
@@ -291,7 +295,7 @@ extern "C" int b200z_file_codec(int op, const char *in_path, uint64_t in_off, ui
                                 uint64_t *out_len) {
   if (in_used) *in_used = 0;
   if (out_len) *out_len = 0;
-  if (op < B200Z_FILE_GZIP_DECODE || op > B200Z_FILE_BZIP2_ENCODE || !in_path || !out_path) {
+  if (op < B200Z_FILE_GZIP_DECODE || op > B200Z_FILE_XZ_ENCODE || !in_path || !out_path) {
     set_error_text("b200z_file_codec: invalid argument");
     return B200Z_E_ARG;
   }

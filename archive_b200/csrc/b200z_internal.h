@@ -148,6 +148,8 @@ cudaError_t deflate_slow_device(const uint8_t *d_in, size_t n, int level, int wi
 cudaError_t deflate_stored_device(const uint8_t *d_in, const DeflStoredBlock *h_blocks, uint32_t n_blocks, uint8_t *d_out,
                                   size_t out_cap, void *ws, size_t ws_bytes, size_t *out_len, cudaStream_t s);
 cudaError_t crc32_tiles_device(const uint8_t *d_in, size_t n, uint32_t tile, uint32_t *d_part, cudaStream_t s);
+// CRC-32 of device bytes d[0, n) on stream s (blocking): tiles of 8 KiB into d_part ((n / 8192 + 1) words), folded on the host
+int device_crc32_on(const uint8_t *d, size_t n, uint32_t *d_part, cudaStream_t s, uint32_t *out);
 
 // ---- encrypted ZIP members (zip_crypt_kernels.cu) ----
 struct ZipAesMember {   // one WinZip AES member; offsets are bytes from the device base pointer of the call
@@ -180,5 +182,13 @@ cudaError_t zip_launch_aes_ctr(const ZipAesMember *d_m, const uint32_t *d_rk, co
 cudaError_t zip_launch_hmac(const ZipAesMember *d_m, uint32_t n, const uint8_t *d_dk, const uint8_t *d_base, bool after_ctr,
                             uint8_t *d_mac, cudaStream_t s);
 cudaError_t zip_launch_zipcrypto(const ZipCryptoMember *d_m, uint32_t n, const uint32_t keys[3], uint8_t *d_base, cudaStream_t s);
+
+// ---- XZ (xz_kernels.cu): host buffers in, host buffers out, blocking on `s` ----
+size_t xz_bound(const uint8_t *in, size_t n);  // the output the container declares, up to where its walk stops
+int xz_decode_impl(const uint8_t *in, size_t n, int verify, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s);
+int xz_crc64_impl(const uint8_t *in, size_t n, uint64_t *crc, cudaStream_t s);
+size_t xz_encode_bound(size_t n);
+int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s);
+void xz_debug(double *lzma_ms, uint32_t *n_runs);  // k_xz_lzma time (CUDA events) and run count of the last decode
 
 }  // namespace b200z

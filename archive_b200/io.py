@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import os
 
-from .codecs import BZip2Decoder, GZipDecoder
+from .codecs import BZip2Decoder, GZipDecoder, XZDecoder
 from .streams import InputFileStream, OutputFileStream
 from .zip import Archive, ArchiveFile, ZipDecoder
 
@@ -77,13 +77,13 @@ def get_input_extension(input_path: str) -> str:
     return os.path.splitext(lower)[1]
 
 
-_EXTENSIONS = ".tar.gz, .tgz, .tar.bz2, .tbz or .zip"
+_EXTENSIONS = ".tar.gz, .tgz, .tar.bz2, .tbz, .tar.xz, .txz or .zip"
 
 
 def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | None = None, password=None) -> list:
     """extractFileToDisk (:160-267).  .zip: ZipDecoder().decodeStream(InputFileStream, password:) and the member loop above.
-    .tar.gz / .tgz / .tar.bz2 / .tbz: the reference decodes into a temporary `temp.tar` with
-    GZipDecoder / BZip2Decoder.decodeStream(InputFileStream, OutputFileStream) (:183-202) and hands that to TarDecoder; here
+    .tar.gz / .tgz / .tar.bz2 / .tbz / .tar.xz / .txz: the reference decodes into a temporary `temp.tar` with
+    GZipDecoder / BZip2Decoder / XZDecoder.decodeStream(InputFileStream, OutputFileStream) (:183-202) and hands that to TarDecoder; here
     the same two stream objects make the library decode file -> file, and the .tar itself is the result (see the module
     text).  Anything else: ValueError, as the reference's ArgumentError."""
     ext = get_input_extension(input_path)
@@ -96,7 +96,7 @@ def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | N
         finally:
             inp.close_sync()
         return extract_archive_to_disk(archive, output_path, buffer_size=buffer_size)
-    if ext in (".tar.gz", ".tgz", ".tar.bz2", ".tbz"):
+    if ext in (".tar.gz", ".tgz", ".tar.bz2", ".tbz", ".tar.xz", ".txz"):
         os.makedirs(output_path, exist_ok=True)
         base = os.path.basename(input_path)
         stem = base[:-len(ext)] if base.lower().endswith(ext) else os.path.splitext(base)[0]
@@ -104,7 +104,7 @@ def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | N
         inp = InputFileStream(input_path)
         out = OutputFileStream(tar_path, buffer_size=buffer_size)
         try:
-            dec = GZipDecoder() if ext in (".tar.gz", ".tgz") else BZip2Decoder()
+            dec = GZipDecoder() if ext in (".tar.gz", ".tgz") else XZDecoder() if ext in (".tar.xz", ".txz") else BZip2Decoder()
             dec.decode_stream(inp, out)  # the reference ignores the bool here too
         finally:
             inp.close_sync()

@@ -64,6 +64,8 @@ const b200zFileBzip2Decode = 3;
 const b200zFileZlibEncode = 4;
 const b200zFileGzipEncode = 5;
 const b200zFileBzip2Encode = 6;
+const b200zFileXzDecode = 7;
+const b200zFileXzEncode = 8;
 typedef _FileCodecC = Int32 Function(Int32 op, Pointer<Utf8> inPath, Uint64 inOff, Uint64 inLen, Pointer<Utf8> outPath,
     Uint64 outOff, Int32 a0, Int32 a1, Uint32 a2, Pointer<Uint64> inUsed, Pointer<Uint64> outLen);
 typedef _FileCodecD = int Function(int op, Pointer<Utf8> inPath, int inOff, int inLen, Pointer<Utf8> outPath, int outOff,
@@ -155,6 +157,8 @@ typedef _Bz2ShardD = int Function(Pointer<Uint8> inp, int inLen, int rank, int w
     Pointer<Size> outLen, Pointer<Bz2Block> blocks, int blocksCap, Pointer<Size> nBlocks);
 typedef _Crc32C = Int32 Function(Pointer<Uint8> inp, Size inLen, Pointer<Uint32> crc);
 typedef _Crc32D = int Function(Pointer<Uint8> inp, int inLen, Pointer<Uint32> crc);
+typedef _Crc64C = Int32 Function(Pointer<Uint8> inp, Size inLen, Pointer<Uint64> crc);
+typedef _Crc64D = int Function(Pointer<Uint8> inp, int inLen, Pointer<Uint64> crc);
 typedef _DeflateBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size nUnits,
     Int32 level, Int32 windowBits, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
     Pointer<Uint32> crc32, Pointer<Int32> status);
@@ -241,6 +245,12 @@ class B200Z {
   late final _ZipAesEncryptD zipAesEncrypt = _lib.lookupFunction<_ZipAesEncryptC, _ZipAesEncryptD>('b200z_zip_aes_encrypt');
   late final _Bz2ShardD bzip2DecodeShard = _lib.lookupFunction<_Bz2ShardC, _Bz2ShardD>('b200z_bzip2_decode_shard');
   late final _Crc32D crc32 = _lib.lookupFunction<_Crc32C, _Crc32D>('b200z_crc32');
+  // XZ: (in, inLen, verify | check, out, cap, outLen) -- the same shape as b200z_bzip2_decode
+  late final _Bz2DecodeD xzDecode = _lib.lookupFunction<_Bz2DecodeC, _Bz2DecodeD>('b200z_xz_decode');
+  late final _BoundD xzBound = _lib.lookupFunction<_BoundC, _BoundD>('b200z_xz_bound');
+  late final _Bz2DecodeD xzEncode = _lib.lookupFunction<_Bz2DecodeC, _Bz2DecodeD>('b200z_xz_encode');
+  late final _SizeOfD xzEncodeBound = _lib.lookupFunction<_SizeOfC, _SizeOfD>('b200z_xz_encode_bound');
+  late final _Crc64D crc64 = _lib.lookupFunction<_Crc64C, _Crc64D>('b200z_crc64');
   late final _DeflateBatchD deflateBatch = _lib.lookupFunction<_DeflateBatchC, _DeflateBatchD>('b200z_deflate_batch');
   late final _InflateBatchD inflateBatch = _lib.lookupFunction<_InflateBatchC, _InflateBatchD>('b200z_inflate_batch');
   late final _InflateBatchDeviceD inflateBatchDevice =

@@ -180,6 +180,54 @@ class BZip2Decoder {
   }
 }
 
+/// `XZDecoder` (xz_decoder.dart:15-27): one stream; the LZMA2 runs between dictionary resets decode on the device.
+class XZDecoder {
+  Uint8List decodeBytes(List<int> data, {bool verify = false}) {
+    final out = ar.OutputMemoryStream();
+    decodeStream(ar.InputMemoryStream(data), out, verify: verify);
+    return out.getBytes();
+  }
+
+  bool decodeStream(ar.InputStream input, ar.OutputStream output, {bool verify = false}) {
+    final viaFiles = _fileToFile(b200zFileXzDecode, input, output, a0: verify ? 1 : 0);
+    if (viaFiles != null) return viaFiles;
+    final z = B200Z.instance;
+    final data = _drain(input);
+    final inp = z.toNative(data);
+    try {
+      final (out, ok) = z.grow(z.xzBound(inp, data.length) + 64,
+          (o, cap, outLen) => z.xzDecode(inp, data.length, verify ? 1 : 0, o, cap, outLen));
+      output.writeBytes(out);
+      input.skip(data.length);
+      return ok;
+    } finally {
+      z.hostFree(inp);
+    }
+  }
+}
+
+/// `XZEncoder` (xz_encoder.dart:18-62): one stored LZMA2 chunk and the check, computed on the device.
+class XZEncoder {
+  Uint8List encodeBytes(List<int> data, {ar.XZCheck check = ar.XZCheck.crc64}) {
+    final z = B200Z.instance;
+    final inp = z.toNative(data);
+    try {
+      final (out, _) = z.grow(z.xzEncodeBound(data.length),
+          (o, cap, outLen) => z.xzEncode(inp, data.length, check.index, o, cap, outLen));
+      return out;
+    } finally {
+      z.hostFree(inp);
+    }
+  }
+
+  List<int> encode(List<int> data, {ar.XZCheck check = ar.XZCheck.crc64}) => encodeBytes(data, check: check);
+
+  void encodeStream(ar.InputStream input, ar.OutputStream output, {ar.XZCheck check = ar.XZCheck.crc64}) {
+    if (_fileToFile(b200zFileXzEncode, input, output, a0: check.index) != null) return;
+    output.writeBytes(encodeBytes(_drain(input), check: check));
+  }
+}
+
 // ---- encoders: the `platformZLibEncoder` / `platformGZipEncoder` seam (_zlib_encoder.dart:1, _gzip_encoder.dart:1),
 // `Deflate` (deflate.dart:25-100) and `BZip2Encoder` (bzip2_encoder.dart:15-81) ----
 

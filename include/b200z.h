@@ -145,6 +145,24 @@ size_t b200z_bzip2_bound(size_t in_len); /* output capacity that always suffices
  * folded with x^(8n) mod P): what ZipEncoder stores for members it does not deflate (zip_encoder.dart:113-134).   */
 int b200z_crc32(const uint8_t *in, size_t in_len, uint32_t *crc);
 
+/* ---- XZ: XZDecoder / XZEncoder (codecs/xz_decoder.dart, codecs/xz_encoder.dart, codecs/lzma/) ------------------------
+ * b200z_xz_decode = XZDecoder().decodeBytes(data, verify:): ONE stream (bytes after its footer are ignored).  The host walks
+ * the container and every LZMA2 chunk header; the runs between dictionary resets are decoded on the device in parallel
+ * (one warp each), stored chunks are copies.  B200Z_OK: decodeStream returned true.  B200Z_E_DATA: it returned false, and
+ * `out` holds the bytes the reference would have written.  B200Z_E_THROW: the reference throws (a read past the input or
+ * a chunk's compressed bytes, a reach before the dictionary, posState >= 12 with pb = 4 or 5, or a match that runs past
+ * its chunk's declared size -- DESIGN.md section 7).  B200Z_E_NOSPC: out_cap is below b200z_xz_bound, *out_len = that.
+ * With `verify`, CRC-32 / CRC-64 block checks are compared (on the device); SHA-256 is read and never compared.
+ * b200z_xz_bound (host only): the output the container declares up to where its walk stops; 0 when it declares none.
+ * b200z_xz_encode = XZEncoder().encodeBytes(data, check:) with check 0 none, 1 crc32, 2 crc64, 3 sha256 (XZCheck.index):
+ * one stored chunk whose 16-bit length field is cut for inputs over 64 KiB, as in the reference.
+ * b200z_crc64 = getCrc64(bytes) (util/_crc64_io.dart: ECMA-182, reflected), tile CRCs on the device folded on the host. */
+int b200z_xz_decode(const uint8_t *in, size_t in_len, int verify, uint8_t *out, size_t out_cap, size_t *out_len);
+size_t b200z_xz_bound(const uint8_t *in, size_t in_len);
+int b200z_xz_encode(const uint8_t *in, size_t in_len, int check, uint8_t *out, size_t out_cap, size_t *out_len);
+size_t b200z_xz_encode_bound(size_t in_len);
+int b200z_crc64(const uint8_t *in, size_t in_len, uint64_t *crc);
+
 /* ---- ZIP container: ZipDecoder / ZipDirectory / ZipFileHeader / ZipFile ------------------------------------
  * b200z_zip_list   = ZipDirectory.read (zip_directory.dart:25-183) + ZipFileHeader.read (zip_file_header.dart:28-111)
  *                    + ZipFile.read (zip_file.dart:73-149), host only: no device is needed.
@@ -226,13 +244,17 @@ int b200z_zip_aes_encrypt(uint8_t *data, const uint64_t *off, const uint64_t *le
  *   B200Z_FILE_BZIP2_DECODE   verify   -            -        BZip2Decoder.decodeStream    (bzip2_decoder.dart:21-88)
  *   B200Z_FILE_ZLIB_ENCODE    level    window_bits  raw      ZLibEncoderWeb.encodeStream  (_zlib_encoder_web.dart:30-73)
  *   B200Z_FILE_GZIP_ENCODE    level    -            mtime    GZipEncoderWeb.encodeStream  (_gzip_encoder_web.dart:30-100)
- *   B200Z_FILE_BZIP2_ENCODE   -        -            -        BZip2Encoder.encodeStream    (bzip2_encoder.dart:25-81)     */
+ *   B200Z_FILE_BZIP2_ENCODE   -        -            -        BZip2Encoder.encodeStream    (bzip2_encoder.dart:25-81)
+ *   B200Z_FILE_XZ_DECODE      verify   -            -        XZDecoder.decodeStream       (xz_decoder.dart:22-26)
+ *   B200Z_FILE_XZ_ENCODE      check    -            -        XZEncoder.encodeStream       (xz_encoder.dart:30-62)       */
 #define B200Z_FILE_GZIP_DECODE 1
 #define B200Z_FILE_ZLIB_DECODE 2
 #define B200Z_FILE_BZIP2_DECODE 3
 #define B200Z_FILE_ZLIB_ENCODE 4
 #define B200Z_FILE_GZIP_ENCODE 5
 #define B200Z_FILE_BZIP2_ENCODE 6
+#define B200Z_FILE_XZ_DECODE 7
+#define B200Z_FILE_XZ_ENCODE 8
 int b200z_file_codec(int op, const char *in_path, uint64_t in_off, uint64_t in_len, const char *out_path, uint64_t out_off,
                      int32_t a0, int32_t a1, uint32_t a2, uint64_t *in_used, uint64_t *out_len);
 /* How the last b200z_file_codec call of this process went: segments decoded through the member-boundary pipeline, and

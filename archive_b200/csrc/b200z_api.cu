@@ -291,8 +291,320 @@ struct OneResult {
 };
 // `shared_output`: the stream is a gzip member -- everything already in g.d_out[0, out_pos) belongs to the same OutputStream
 // and is within reach of its back-references (InflateWs::hist)
-static int run_one_staged(size_t pos, size_t in_total, size_t out_pos, size_t out_cap_total, OneResult *r,
-                          bool shared_output = false) {
+// ---------------------------------------------------------------------------------------------
+// K12: one stream decoded by many chunks (inflate_chunked.cuh, DESIGN.md "K12").  The stream's compressed input is
+// worked through in regions that double from g_ck.thresh bytes: per region the block finder guesses a block start in
+// every chunk, all chunks decode at once, the chain is proven on the host from the region's exact start and the chunks
+// that started at a wrong guess are redone from their predecessor's end; then the windows are resolved and the region
+// is written to its final place.  The result is accepted only when the chain reaches a final block with every chunk
+// on it clean, no back-reference reaches before the allowed history and the output fits the cap; anything else leaves
+// the stream to the exact single-unit path, which gives every other result exactly.
+// ---------------------------------------------------------------------------------------------
+// Compressed bytes from which a stream takes K12, and the chunk size (0: a region's bytes over CK_TARGET, at least
+// CK_MIN_CHUNK).  Both are set by the benchmark's measurements (DESIGN.md "K12"); b200z_debug_inflate_chunked_set moves them
+// for tests.
+constexpr size_t CK_THRESH = 16u << 20;
+constexpr size_t CK_MIN_CHUNK = 32u << 10;
+constexpr size_t CK_TARGET = 2048;
+constexpr int CK_MAX_ROUNDS = 16;  // redo rounds per region before the stream goes to the exact path
+struct CkConfig {
+  size_t thresh = CK_THRESH, chunk = 0;
+};
+static CkConfig g_ck;
+static unsigned long long g_ck_stats[6];  // last call: regions, chunks, redo rounds, chunks merged, fell back, chunked path ran
+static double g_ck_ms[3];  // last call's kernel times (CUDA events): block finder, chunk decodes (all rounds), windows + emit
+// Times the kernels of one phase of run_chunked on g.stream; the phase's own synchronisation makes the reading cheap.
+struct CkTimer {
+  cudaEvent_t a = nullptr, b = nullptr;
+  CkTimer() {
+    cudaEventCreate(&a);
+    cudaEventCreate(&b);
+  }
+  ~CkTimer() {
+    cudaEventDestroy(a);
+    cudaEventDestroy(b);
+  }
+  void start() { cudaEventRecord(a, g.stream); }
+  void stop(double *acc) {
+    cudaEventRecord(b, g.stream);
+    float ms = 0.f;
+    if (cudaEventSynchronize(b) == cudaSuccess && cudaEventElapsedTime(&ms, a, b) == cudaSuccess) *acc += ms;
+  }
+};
+
+static size_t ck_carve(size_t &o, size_t bytes) {
+  const size_t at = o;
+  o = align_up(o + bytes, 256);
+  return at;
+}
+
+// Returns B200Z_OK with *accepted set when K12 produced the stream's result; an error code only for CUDA failures.
+static int run_chunked(const uint8_t *h_in, size_t pos, uint32_t il, size_t out_pos, uint32_t oc, uint32_t hist, OneResult *r,
+                       bool *accepted) {
+  *accepted = false;
+  for (auto &v : g_ck_stats) v = 0;
+  g_ck_stats[5] = 1;
+  CkTimer tm;
+  const uint8_t *in = (const uint8_t *)g.d_in.p + pos;
+  // the exact path's workspace for the same call: the pool is carved from it
+  const size_t ws = workspace_bytes(1, out_pos + oc);
+  CU(g.d_ws.reserve(ws));
+  const size_t max_ch = CK_TARGET + 8;
+  size_t o = 0;
+  const size_t o_lo = ck_carve(o, max_ch * 8), o_hi = ck_carve(o, max_ch * 8), o_cand = ck_carve(o, max_ch * 8);
+  const size_t o_jobs = ck_carve(o, max_ch * sizeof(CkJob)), o_res = ck_carve(o, max_ch * sizeof(CkRes));
+  const size_t o_chain = ck_carve(o, max_ch * sizeof(CkChain)), o_ctr = ck_carve(o, 16);
+  const size_t fixed = o;
+  // page records, the flat page list and the pages, plus the alignment the carving below may add (three times 256)
+  const size_t per_page = (size_t)CK_PAGE * 2 + sizeof(CkPage) + 8;
+  if (ws < fixed + 1024 + 8 * per_page) {  // (checked before the subtraction: a small cap gives a small workspace)
+    g_ck_stats[4] = 1;
+    return B200Z_OK;
+  }
+  const size_t n_pages_sz = (ws - fixed - 1024) / per_page;
+  const uint32_t n_pages = (uint32_t)std::min<size_t>(n_pages_sz, 0xffffffu);
+  const size_t o_pinfo = ck_carve(o, (size_t)n_pages * sizeof(CkPage)), o_flat = ck_carve(o, (size_t)n_pages * 8);
+  const size_t o_pool = ck_carve(o, (size_t)n_pages * CK_PAGE * 2);
+  uint8_t *w = (uint8_t *)g.d_ws.p;
+  auto *d_lo = (unsigned long long *)(w + o_lo), *d_hi = (unsigned long long *)(w + o_hi), *d_cand = (unsigned long long *)(w + o_cand);
+  auto *d_jobs = (CkJob *)(w + o_jobs);
+  auto *d_res = (CkRes *)(w + o_res);
+  auto *d_chain = (CkChain *)(w + o_chain);
+  auto *d_ctr = (uint32_t *)(w + o_ctr);
+  auto *d_pinfo = (CkPage *)(w + o_pinfo);
+  auto *d_flat = (uint32_t *)(w + o_flat);
+  auto *d_pool = (uint16_t *)(w + o_pool);
+  uint8_t *d_out = (uint8_t *)g.d_out.p;
+  const unsigned long long lo_valid = out_pos - hist;
+  const unsigned long long end_bits = 8ull * il;
+  // A block that is not final starts at `e` with a stored header that reads the same LEN / NLEN as the one found at `c`:
+  // bits e .. e + 2 are 000 and both reach the same byte boundary.
+  auto bit_at = [&](unsigned long long b) { return b < end_bits ? (h_in[b >> 3] >> (b & 7)) & 1u : 1u; };
+  auto stored_alike = [&](unsigned long long e, unsigned long long c) {
+    return ((e + 10) >> 3) == ((c + 10) >> 3) && bit_at(e) == 0 && bit_at(e + 1) == 0 && bit_at(e + 2) == 0;
+  };
+
+  if (bit_at(1) == 0 && bit_at(2) == 0) {  // a stream that opens with a stored block: incompressible data, see below
+    g_ck_stats[4] = 1;
+    return B200Z_OK;
+  }
+  unsigned long long bit0 = 0;  // the region's exact start
+  size_t emitted = 0, R = g_ck.thresh;
+  std::vector<unsigned long long> S, lo, hi, cand;
+  std::vector<CkJob> jobs, redo;
+  std::vector<CkRes> res;
+  std::vector<CkPage> pinfo;
+  std::vector<CkChain> chain;
+  std::vector<uint32_t> flat, flat_chunk, on_chain;
+  for (;;) {
+    g_ck_stats[0]++;
+    const size_t b0 = (size_t)(bit0 >> 3);
+    const size_t rend = std::min<size_t>(il, b0 + R);
+    const size_t span = rend - b0;
+    size_t C = g_ck.chunk ? g_ck.chunk : std::max<size_t>(CK_MIN_CHUNK, (span + CK_TARGET - 1) / CK_TARGET);
+    size_t n = std::max<size_t>(1, (span + C - 1) / C);
+    if (n > CK_TARGET) {
+      C = (span + CK_TARGET - 1) / CK_TARGET;
+      n = (span + C - 1) / C;
+    }
+    // ---- nominal chunk starts, and a block start guessed in each (chunk 0 starts at the proven bit0) ----
+    S.assign(n + 1, 0);
+    S[0] = bit0;
+    for (size_t k = 1; k < n; ++k) S[k] = 8ull * (b0 + k * C);
+    S[n] = rend == il ? ~0ull : 8ull * rend;
+    cand.assign(n, CK_NOCAND);
+    cand[0] = bit0;
+    if (n > 1) {
+      lo.assign(S.begin() + 1, S.begin() + n);
+      hi.assign(S.begin() + 2, S.begin() + n + 1);
+      if (hi.back() > end_bits) hi.back() = end_bits;
+      CU(cudaMemcpyAsync(d_lo, lo.data(), lo.size() * 8, cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemcpyAsync(d_hi, hi.data(), hi.size() * 8, cudaMemcpyHostToDevice, g.stream));
+      tm.start();
+      CU(ck_launch_find(in, il, d_lo, d_hi, d_cand, (uint32_t)(n - 1), g.stream));
+      tm.stop(&g_ck_ms[0]);
+      CU(cudaMemcpyAsync(cand.data() + 1, d_cand, (n - 1) * 8, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaStreamSynchronize(g.stream));
+    }
+    // ---- a chunk without a candidate is merged into its predecessor: jobs[i] covers up to the next kept start ----
+    jobs.clear();
+    for (size_t k = 0; k < n; ++k)
+      if (cand[k] != CK_NOCAND) jobs.push_back(CkJob{cand[k], 0, (uint32_t)jobs.size(), 0});
+    const size_t nj = jobs.size();
+    {
+      size_t i = 0;
+      for (size_t k = 0; k < n; ++k) {
+        if (cand[k] == CK_NOCAND) continue;
+        size_t k2 = k + 1;
+        while (k2 < n && cand[k2] == CK_NOCAND) ++k2;
+        jobs[i++].stop_bit = S[k2];
+      }
+    }
+    g_ck_stats[1] += nj;
+    g_ck_stats[3] += n - nj;
+    // No block start found in a whole MiB (fixed-Huffman streams look like noise to the finder; stored blocks hold at most
+    // 64 KiB and zlib's dynamic ones far less): one lane would walk all of it, slower than the exact path's warp.
+    if (nj == 1 && span >= (1u << 20)) {
+      g_ck_stats[4] = 1;
+      return B200Z_OK;
+    }
+    // Mostly stored blocks (incompressible data): the exact path moves a stored block as one run of bytes, where a chunk
+    // lane copies it symbol by symbol; measured slower here (DESIGN.md "K12"), so such a stream stays on the exact path.
+    {
+      size_t n_stored = 0;
+      for (const CkJob &jb : jobs) {
+        const size_t at = (size_t)((jb.start_bit + 10) >> 3);  // LEN of a stored block starting there
+        n_stored += bit_at(jb.start_bit + 1) == 0 && bit_at(jb.start_bit + 2) == 0 && at + 2 <= il &&
+                    (h_in[at] | (h_in[at + 1] << 8)) >= 1024;  // (flush markers are empty stored blocks)
+      }
+      if (nj >= 8 && 2 * n_stored > nj) {
+        g_ck_stats[4] = 1;
+        return B200Z_OK;
+      }
+    }
+    CU(cudaMemsetAsync(d_ctr, 0, 4, g.stream));
+    CU(cudaMemcpyAsync(d_jobs, jobs.data(), nj * sizeof(CkJob), cudaMemcpyHostToDevice, g.stream));
+    tm.start();
+    CU(ck_launch_chunks(in, il, d_jobs, (uint32_t)nj, d_res, d_pool, d_pinfo, d_ctr, n_pages, g.stream));
+    tm.stop(&g_ck_ms[1]);
+    res.resize(nj);
+    CU(cudaMemcpyAsync(res.data(), d_res, nj * sizeof(CkRes), cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+    // ---- prove the chain from bit0; redo what started at a wrong guess ----
+    bool final_seen = false;
+    unsigned long long pos_b = bit0;
+    on_chain.clear();
+    for (int round = 0;; ++round) {
+      pos_b = bit0;
+      on_chain.clear();
+      final_seen = false;
+      size_t bad_at = nj;
+      for (size_t i = 0; i < nj; ++i) {
+        if (i > 0 && pos_b >= jobs[i].stop_bit) continue;  // its whole slice lies inside its predecessor's last block
+        if (jobs[i].start_bit != pos_b && res[i].first_stored && stored_alike(pos_b, jobs[i].start_bit))
+          jobs[i].start_bit = pos_b;  // the same stored block read from its true header: the same result
+        if (jobs[i].start_bit != pos_b) {
+          bad_at = i;
+          break;
+        }
+        const int st = res[i].status;
+        if (st != CK_BOUNDARY && st != CK_FINAL) {  // the exact step fails here too (or the pool ran out)
+          g_ck_stats[4] = 1;
+          return B200Z_OK;
+        }
+        on_chain.push_back((uint32_t)i);
+        pos_b = res[i].end_bit;
+        if (st == CK_FINAL) {
+          final_seen = true;
+          break;
+        }
+      }
+      if (bad_at == nj) break;
+      if (round >= CK_MAX_ROUNDS) {
+        g_ck_stats[4] = 1;
+        return B200Z_OK;
+      }
+      // Redo the first unproven chunk from the proven end and, together with it, every later chunk that does not start
+      // where its predecessor's last attempt ended (from that end: usually right, and proven or redone next round).
+      redo.clear();
+      std::vector<size_t> redo_idx;
+      unsigned long long prev_end = pos_b;
+      for (size_t i = bad_at; i < nj; ++i) {
+        if (prev_end >= jobs[i].stop_bit) continue;  // empty: the end carries over
+        const bool mism = jobs[i].start_bit != prev_end &&
+                          !(res[i].first_stored && stored_alike(prev_end, jobs[i].start_bit));
+        if (mism) {
+          jobs[i].start_bit = prev_end;
+          jobs[i].gen++;
+          redo.push_back(jobs[i]);
+          redo_idx.push_back(i);
+        }
+        if (res[i].status != CK_BOUNDARY) break;
+        prev_end = res[i].end_bit;
+      }
+      g_ck_stats[2]++;
+      CU(cudaMemcpyAsync(d_jobs, redo.data(), redo.size() * sizeof(CkJob), cudaMemcpyHostToDevice, g.stream));
+      tm.start();
+      CU(ck_launch_chunks(in, il, d_jobs, (uint32_t)redo.size(), d_res, d_pool, d_pinfo, d_ctr, n_pages, g.stream));
+      tm.stop(&g_ck_ms[1]);
+      std::vector<CkRes> rr(redo.size());
+      CU(cudaMemcpyAsync(rr.data(), d_res, rr.size() * sizeof(CkRes), cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaStreamSynchronize(g.stream));
+      for (size_t q = 0; q < redo.size(); ++q) res[redo_idx[q]] = rr[q];
+    }
+    if (!final_seen && rend == il) {  // the input ends without a final block: the exact step's EOS / STOP
+      g_ck_stats[4] = 1;
+      return B200Z_OK;
+    }
+    // ---- output offsets, the chain's pages in order, then windows and bytes ----
+    uint32_t pages_used = 0;
+    CU(cudaMemcpyAsync(&pages_used, d_ctr, 4, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+    pages_used = std::min(pages_used, n_pages);
+    pinfo.resize(pages_used);
+    if (pages_used) CU(cudaMemcpyAsync(pinfo.data(), d_pinfo, pages_used * sizeof(CkPage), cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+    chain.clear();
+    std::vector<uint32_t> slot_to_chain(nj, 0xffffffffu);
+    size_t total = 0, nflat = 0;
+    for (uint32_t i : on_chain) {
+      slot_to_chain[i] = (uint32_t)chain.size();
+      chain.push_back(CkChain{(unsigned long long)(out_pos + emitted + total), res[i].nsym, (uint32_t)nflat});
+      total += res[i].nsym;
+      nflat += (res[i].nsym + CK_PAGE - 1) / CK_PAGE;
+    }
+    if (emitted + total > oc) {  // the exact path's NOSPC
+      g_ck_stats[4] = 1;
+      return B200Z_OK;
+    }
+    flat.assign(nflat, 0xffffffffu);
+    flat_chunk.assign(nflat, 0);
+    for (uint32_t p = 0; p < pages_used; ++p) {
+      const CkPage &pi = pinfo[p];
+      if (pi.slot >= nj || slot_to_chain[pi.slot] == 0xffffffffu || pi.gen != jobs[pi.slot].gen) continue;
+      const CkChain &c = chain[slot_to_chain[pi.slot]];
+      if ((size_t)pi.seq * CK_PAGE >= c.nsym) continue;
+      flat[c.page0 + pi.seq] = p;
+      flat_chunk[c.page0 + pi.seq] = slot_to_chain[pi.slot];
+    }
+    for (uint32_t f : flat)
+      if (f == 0xffffffffu) {  // (cannot happen: every symbol of a clean chunk is on a page)
+        g_ck_stats[4] = 1;
+        return B200Z_OK;
+      }
+    if (!chain.empty()) {
+      CU(cudaMemcpyAsync(d_chain, chain.data(), chain.size() * sizeof(CkChain), cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemcpyAsync(d_flat, flat.data(), nflat * 4, cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemcpyAsync(d_flat + nflat, flat_chunk.data(), nflat * 4, cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemsetAsync(d_ctr + 1, 0, 4, g.stream));
+      tm.start();
+      CU(ck_launch_resolve(d_chain, (uint32_t)chain.size(), d_flat, d_flat + nflat, (uint32_t)nflat, d_pool, d_out, lo_valid,
+                           d_ctr + 1, g.stream));
+      tm.stop(&g_ck_ms[2]);
+      uint32_t bad = 0;
+      CU(cudaMemcpyAsync(&bad, d_ctr + 1, 4, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaStreamSynchronize(g.stream));
+      if (bad) {  // a back-reference before the allowed history: the exact path's RANGE
+        g_ck_stats[4] = 1;
+        return B200Z_OK;
+      }
+    }
+    emitted += total;
+    if (final_seen) {
+      r->out_len = (uint32_t)emitted;
+      r->in_used = (uint32_t)((pos_b + 7) >> 3);
+      r->status = B200Z_U_DONE;
+      *accepted = true;
+      return B200Z_OK;
+    }
+    bit0 = pos_b;
+    R *= 2;
+  }
+}
+
+// `try_chunked`: K12 may take the stream (the caller knows nothing that makes it pointless)
+static int run_one_staged(const uint8_t *h_in, size_t pos, size_t in_total, size_t out_pos, size_t out_cap_total, OneResult *r,
+                          bool shared_output = false, bool try_chunked = true) {
   uint64_t io = pos, oo = out_pos;
   size_t avail_in = in_total - pos;
   uint32_t il = (uint32_t)(avail_in > 0xfffffff0u ? 0xfffffff0u : avail_in);
@@ -302,6 +614,13 @@ static int run_one_staged(size_t pos, size_t in_total, size_t out_pos, size_t ou
   uint32_t oc = (uint32_t)(room > 0xfffffff0u ? 0xfffffff0u : room);
   CU(g.d_out.reserve_keep(out_pos + oc + 64, out_pos, g.stream));
   const uint32_t hist = shared_output ? (uint32_t)(out_pos > 65535 ? 65535 : out_pos) : 0u;  // distances end at 32768
+  for (auto &v : g_ck_stats) v = 0;
+  for (auto &v : g_ck_ms) v = 0;
+  if (try_chunked && il >= g_ck.thresh) {
+    bool accepted = false;
+    int rc = run_chunked(h_in + pos, pos, il, out_pos, oc, hist, r, &accepted);
+    if (rc || accepted) return rc;
+  }
   return run_batch_on_staged(&io, &il, &oo, &oc, &r->out_len, &r->status, &r->in_used, 1, out_pos + oc, false, hist);
 }
 
@@ -377,6 +696,22 @@ static size_t hinted_run(const uint8_t *in, size_t n, size_t pos, std::vector<Hi
   return p;
 }
 
+// Is there a gzip member header (1f 8b 08, no reserved flag bits, a known XFL and OS byte) in in[from, from + span)?  Only
+// a hint of where the member that starts before `from` ends: chance hits in compressed data are about 2^-38 per byte.
+static bool gzip_member_header_within(const uint8_t *in, size_t n, size_t from, size_t span) {
+  const size_t end = std::min(n, from + span);
+  for (size_t p = from; p + 10 <= end;) {
+    const void *q = memchr(in + p, 0x1f, end - 9 - p);
+    if (!q) return false;
+    p = (size_t)((const uint8_t *)q - in);
+    const uint8_t *h = in + p;
+    if (h[1] == 0x8b && h[2] == 8 && (h[3] & 0xe0) == 0 && (h[8] == 0 || h[8] == 2 || h[8] == 4) && (h[9] <= 13 || h[9] == 255))
+      return true;
+    ++p;
+  }
+  return false;
+}
+
 // GZip member loop on staged input.
 static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size_t out_cap, size_t *out_len_total,
                               size_t pos = 0, size_t out_pos = 0) {
@@ -438,7 +773,10 @@ static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size
       return zlib_decode_staged(in, in_len, pos, verify & B200Z_GZIP_VERIFY, (verify & B200Z_GZIP_RAW) != 0, /*big_endian=*/0, out_pos,
                                 out_cap, out_len_total);  // decodeStream(input, output, verify: verify, raw: raw)
     OneResult r;
-    int rc = run_one_staged(hdr_end, in_len, out_pos, out_cap, &r, /*shared_output=*/true);
+    // A member's input runs to the end of the file, so K12 would work through a whole region of g_ck.thresh bytes for a
+    // small member.  A member whose successor's header shows up closer than that is small: it takes the exact path.
+    int rc = run_one_staged(in, hdr_end, in_len, out_pos, out_cap, &r, /*shared_output=*/true,
+                            !gzip_member_header_within(in, in_len, hdr_end, g_ck.thresh));
     if (rc) return rc;
     out_pos += r.out_len;
     *out_len_total = out_pos;
@@ -859,7 +1197,7 @@ static int zlib_decode_staged(const uint8_t *in, size_t in_len, size_t pos, int 
     pending = 0;
     *out_len_total = committed;
     OneResult r;
-    int rc = run_one_staged(pos, in_len, committed, out_cap, &r);
+    int rc = run_one_staged(in, pos, in_len, committed, out_cap, &r);
     if (rc) return rc;
     if (r.status == B200Z_U_NOSPC) {
       *out_len_total = committed + r.out_len;
@@ -2448,6 +2786,21 @@ extern "C" void b200z_debug_zip_crypt_ms(double out[4]) {
   for (int k = 0; k < 4; ++k) out[k] = g_crypt_ms[k];
 }
 
+// (test hooks, not part of the ABI) K12's threshold and chunk size in compressed bytes (0 each: the built-in values), and
+// the last single-stream call's statistics: regions, chunks, redo rounds, chunks merged, fell back to the exact path,
+// chunked path ran
+extern "C" void b200z_debug_inflate_chunked_set(unsigned long long thresh, unsigned long long chunk) {
+  g_ck.thresh = thresh ? (size_t)thresh : CK_THRESH;
+  g_ck.chunk = (size_t)chunk;
+}
+extern "C" void b200z_debug_inflate_chunked_stats(unsigned long long out[6]) {
+  for (int k = 0; k < 6; ++k) out[k] = g_ck_stats[k];
+}
+// (test hook) the last single-stream call's K12 kernel times in ms (CUDA events): finder, chunk decodes, windows + emit
+extern "C" void b200z_debug_inflate_chunked_ms(double out[3]) {
+  for (int k = 0; k < 3; ++k) out[k] = g_ck_ms[k];
+}
+
 extern "C" {
 
 const char *b200z_version(void) { return "b200z 0.1 (sm_90a)"; }
@@ -2702,7 +3055,7 @@ int b200z_inflate_raw(const uint8_t *in, size_t in_len, uint8_t *out, size_t out
   if (rc) return rc;
   OneResult r{0, 0, B200Z_U_EOS};
   if (in_len > 0) {
-    rc = run_one_staged(0, in_len, 0, out_cap, &r);
+    rc = run_one_staged(in, 0, in_len, 0, out_cap, &r);
     if (rc) return rc;
     if (r.out_len) CU(cudaMemcpyAsync(out, g.d_out.p, r.out_len, cudaMemcpyDeviceToHost, g.stream));
     CU(cudaStreamSynchronize(g.stream));

@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../include/b200z.h"
+#include "inflate_chunked.h"
 
 #ifndef B200Z_LBITS
 #define B200Z_LBITS 9  // literal/length primary LUT bits (2^9 x u16 per stream)
@@ -57,6 +58,14 @@ struct InflateBatch {
 };
 
 cudaError_t launch_inflate(const InflateBatch &b, cudaStream_t stream);
+// K12 (inflate_chunked.cuh)
+cudaError_t ck_launch_find(const uint8_t *in, uint32_t in_len, const unsigned long long *lo, const unsigned long long *hi,
+                           unsigned long long *cand, uint32_t n, cudaStream_t s);
+cudaError_t ck_launch_chunks(const uint8_t *in, uint32_t in_len, const CkJob *jobs, uint32_t n, CkRes *res, uint16_t *pool,
+                             CkPage *pinfo, uint32_t *page_ctr, uint32_t n_pages, cudaStream_t s);
+cudaError_t ck_launch_resolve(const CkChain *chain, uint32_t n_chain, const uint32_t *flat, const uint32_t *flat_chunk,
+                              uint32_t n_flat, const uint16_t *pool, uint8_t *out, unsigned long long lo_valid, uint32_t *bad,
+                              cudaStream_t s);
 cudaError_t launch_find_markers(const uint8_t *d_in, size_t n, unsigned long long *d_list, uint32_t *d_count, uint32_t cap,
                                 cudaStream_t stream);
 

@@ -339,6 +339,93 @@ B200Z_HD int slow_decode(uint32_t bits15, const uint16_t *first, const uint16_t 
 }
 
 // ---------------------------------------------------------------------------------------------
+// Block header after BTYPE: the fixed tables (inflate.dart:408-735) or a dynamic header (inflate.dart:239-298, _decode
+// :345-401) read from `br`, and the block's lit/len and distance tables built (LUTs + SlowTab / SlowTabD; the dynamic
+// ones with the second-level pool behind lut_d).  `lens` (>= 320 entries) is left holding the code lengths.  Returns 0,
+// or the status the exact step stops with: U_STOP_SHORT (a short read), B200Z_U_STOP, B200Z_U_BADCODE, B200Z_U_THROW.
+// Shared by the exact step below and K12's block finder (inflate_chunked.cuh).
+// ---------------------------------------------------------------------------------------------
+constexpr int U_STOP_SHORT = -100;  // internal: B200Z_U_STOP because a read ran out of input (reported as B200Z_U_STOP)
+B200Z_HD int parse_tables(BitReader &br, uint32_t type, uint8_t *lens, uint16_t *lut_l, uint16_t *lut_d, SlowTab &sl,
+                          SlowTabD &sd) {
+  if (type == 1) {
+    for (int i = 0; i < 288; ++i) lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
+    build_table<LBITS, uint16_t>(lens, 288, lut_l, sl.first, sl.count, sl.offs, sl.perm, &sl.maxlen, 256, 285);
+    for (int i = 0; i < 30; ++i) lens[i] = 5;
+    build_table<DBITS, uint8_t>(lens, 30, lut_d, sd.first, sd.count, sd.offs, sd.perm, &sd.maxlen, -1, 29);
+    return 0;
+  }
+  int hlit = br.read_bits_checked(5);
+  if (hlit < 0) return U_STOP_SHORT;
+  hlit += 257;
+  if (hlit > 288) return B200Z_U_STOP;
+  int hdist = br.read_bits_checked(5);
+  if (hdist < 0) return U_STOP_SHORT;
+  hdist += 1;
+  if (hdist > 32) return B200Z_U_STOP;
+  int hclen = br.read_bits_checked(4);
+  if (hclen < 0) return U_STOP_SHORT;
+  hclen += 4;
+  if (hclen > 19) return B200Z_U_STOP;
+  for (int i = 0; i < 19; ++i) lens[i] = 0;
+  for (int i = 0; i < hclen; ++i) {
+    int l = br.read_bits_checked(3);
+    if (l < 0) return U_STOP_SHORT;
+    lens[c_order[i]] = (uint8_t)l;
+  }
+  // code-length alphabet: 7-bit LUT in the (not yet built) lit/len LUT area
+  uint8_t clmax;
+  {
+    uint16_t f[16], c[16], o[16];
+    uint8_t pm[19];
+    if (!build_table<7, uint8_t>(lens, 19, lut_l, f, c, o, pm, &clmax)) return B200Z_U_BADCODE;
+  }
+  // _decode (inflate.dart:345-401)
+  const int num = hlit + hdist;
+  int i = 0, prev = 0;
+  while (i < num) {
+    br.refill();
+    if (!br.fast() && br.rem_bits() < clmax) return U_STOP_SHORT;
+    uint32_t e = lut_l[br.peek(7)];
+    int l = e & 15;
+    int code = e >> 4;
+    // l == 0: hole in an incomplete set -- the reference's flat table yields (len 0, sym 0)
+    // (_huffman_table.dart:22), i.e. a zero length for this symbol and no bits consumed.
+    br.drop(l);
+    int repeat;
+    if (code < 16) {
+      lens[i++] = (uint8_t)code;
+      prev = code;
+      continue;
+    } else if (code == 16) {
+      repeat = br.read_bits_checked(2);
+      if (repeat < 0) return U_STOP_SHORT;
+      repeat += 3;
+    } else if (code == 17) {
+      repeat = br.read_bits_checked(3);
+      if (repeat < 0) return U_STOP_SHORT;
+      repeat += 3;
+      prev = 0;
+    } else {
+      repeat = br.read_bits_checked(7);
+      if (repeat < 0) return U_STOP_SHORT;
+      repeat += 11;
+      prev = 0;
+    }
+    if (i + repeat > num) return B200Z_U_THROW;
+    for (int k = 0; k < repeat; ++k) lens[i++] = (uint8_t)prev;
+  }
+  for (int k = hdist; k < 32; ++k) lens[hlit + k] = 0;
+  uint16_t *sub_p = lut_d + (1 << DBITS);  // second-level pool
+  int sub_used = 0;
+  for (int k = 0; k < SUBN / 2; ++k) reinterpret_cast<uint32_t *>(sub_p)[k] = 0;
+  bool ok = build_table<DBITS, uint8_t>(lens + hlit, hdist, lut_d, sd.first, sd.count, sd.offs, sd.perm, &sd.maxlen, -1, 29, sub_p, SUBN, &sub_used);
+  ok = build_table<LBITS, uint16_t>(lens, hlit, lut_l, sl.first, sl.count, sl.offs, sl.perm, &sl.maxlen, 256, 285, sub_p, SUBN, &sub_used) && ok;
+  if (!ok) return B200Z_U_BADCODE;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
 // One stream: DEFLATE bits -> token stream.  Runs as one LANE of k_inflate_decode (and, compiled as
 // plain C++, inside tests/host_emul to check the logic against the oracle without a GPU).
 // ---------------------------------------------------------------------------------------------
@@ -366,7 +453,6 @@ constexpr int SPEC_HSHIFT = 2;         // helper token region = unit capacity >>
 constexpr int PIECE_MAX = 30;
 constexpr int PIECE_WORDS = 2 + 3 * PIECE_MAX;  // [0] = count, then (src, start, count) from word 2: src 0 = own region, k = helper k
 constexpr int USCRATCH_BYTES = (SPEC_MAX_G - 1) * SPEC_BMW * 4;  // per unit: the helpers' boundary bitmaps
-constexpr int U_STOP_SHORT = -100;  // internal: B200Z_U_STOP because a read ran out of input (reported as B200Z_U_STOP)
 constexpr uint32_t SPEC_BIAS = 0x40000000u;  // helpers count output bytes from here, so "distance > produced" never fires
 constexpr uint32_t SPEC_NOLINK = 0xffffffffu;
 
@@ -826,84 +912,9 @@ B200Z_HD UnitResult inflate_decode_unit(bool active, const uint8_t *in, uint32_t
         }
         br.seek(pos + (uint32_t)len);
         break;  // next token
-      } else if (type == 1) {
-        // ---- fixed tables (inflate.dart:408-735): 288 lit/len lengths, 30 distance lengths ----
-        for (int i = 0; i < 288; ++i) lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
-        build_table<LBITS, uint16_t>(lens, 288, lut_l, sl.first, sl.count, sl.offs, sl.perm, &sl.maxlen, 256, 285);
-        for (int i = 0; i < 30; ++i) lens[i] = 5;
-        build_table<DBITS, uint8_t>(lens, 30, lut_d, sd.first, sd.count, sd.offs, sd.perm, &sd.maxlen, -1, 29);
-      } else if (type == 2) {
-        // ---- dynamic (inflate.dart:239-298) ----
-        int hlit = br.read_bits_checked(5);
-        if (hlit < 0) { st = U_STOP_SHORT; done = true; break; }
-        hlit += 257;
-        if (hlit > 288) { st = B200Z_U_STOP; done = true; break; }
-        int hdist = br.read_bits_checked(5);
-        if (hdist < 0) { st = U_STOP_SHORT; done = true; break; }
-        hdist += 1;
-        if (hdist > 32) { st = B200Z_U_STOP; done = true; break; }
-        int hclen = br.read_bits_checked(4);
-        if (hclen < 0) { st = U_STOP_SHORT; done = true; break; }
-        hclen += 4;
-        if (hclen > 19) { st = B200Z_U_STOP; done = true; break; }
-        for (int i = 0; i < 19; ++i) lens[i] = 0;
-        bool bad = false;
-        for (int i = 0; i < hclen; ++i) {
-          int l = br.read_bits_checked(3);
-          if (l < 0) { bad = true; break; }
-          lens[c_order[i]] = (uint8_t)l;
-        }
-        if (bad) { st = U_STOP_SHORT; done = true; break; }
-        // code-length alphabet: 7-bit LUT in the (not yet built) lit/len LUT area
-        uint8_t clmax;
-        {
-          uint16_t f[16], c[16], o[16];
-          uint8_t pm[19];
-          if (!build_table<7, uint8_t>(lens, 19, lut_l, f, c, o, pm, &clmax)) { st = B200Z_U_BADCODE; done = true; break; }
-        }
-        // _decode (inflate.dart:345-401)
-        const int num = hlit + hdist;
-        int i = 0, prev = 0;
-        int err = 0;
-        while (i < num) {
-          br.refill();
-          if (!br.fast() && br.rem_bits() < clmax) { err = U_STOP_SHORT; break; }
-          uint32_t e = lut_l[br.peek(7)];
-          int l = e & 15;
-          int code = e >> 4;
-          // l == 0: hole in an incomplete set -- the reference's flat table yields (len 0, sym 0)
-          // (_huffman_table.dart:22), i.e. a zero length for this symbol and no bits consumed.
-          br.drop(l);
-          int repeat;
-          if (code < 16) {
-            lens[i++] = (uint8_t)code;
-            prev = code;
-            continue;
-          } else if (code == 16) {
-            repeat = br.read_bits_checked(2);
-            if (repeat < 0) { err = U_STOP_SHORT; break; }
-            repeat += 3;
-          } else if (code == 17) {
-            repeat = br.read_bits_checked(3);
-            if (repeat < 0) { err = U_STOP_SHORT; break; }
-            repeat += 3;
-            prev = 0;
-          } else {
-            repeat = br.read_bits_checked(7);
-            if (repeat < 0) { err = U_STOP_SHORT; break; }
-            repeat += 11;
-            prev = 0;
-          }
-          if (i + repeat > num) { err = B200Z_U_THROW; break; }
-          for (int k = 0; k < repeat; ++k) lens[i++] = (uint8_t)prev;
-        }
-        if (err) { st = err; done = true; break; }
-        for (int k = hdist; k < 32; ++k) lens[hlit + k] = 0;
-        int sub_used = 0;
-        for (int k = 0; k < SUBN / 2; ++k) reinterpret_cast<uint32_t *>(sub_p)[k] = 0;
-        bool ok = build_table<DBITS, uint8_t>(lens + hlit, hdist, lut_d, sd.first, sd.count, sd.offs, sd.perm, &sd.maxlen, -1, 29, sub_p, SUBN, &sub_used);
-        ok = build_table<LBITS, uint16_t>(lens, hlit, lut_l, sl.first, sl.count, sl.offs, sl.perm, &sl.maxlen, 256, 285, sub_p, SUBN, &sub_used) && ok;
-        if (!ok) { st = B200Z_U_BADCODE; done = true; break; }
+      } else if (type == 1 || type == 2) {
+        const int pst = parse_tables(br, type, lens, lut_l, lut_d, sl, sd);
+        if (pst != 0) { st = pst; done = true; break; }
       } else {
         st = B200Z_U_STOP;
         done = true; break;

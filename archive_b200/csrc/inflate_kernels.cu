@@ -36,6 +36,7 @@ struct InflateWs {
 #endif
 #include "inflate_decode.cuh"
 #include "inflate_fast.cuh"
+#include "inflate_chunked.cuh"
 
 #include <stdlib.h>
 
@@ -389,6 +390,34 @@ cudaError_t launch_find_markers(const uint8_t *d_in, size_t n, unsigned long lon
   if (e != cudaSuccess || n == 0) return e;
   const unsigned long long threads = (n + 15) / 16;
   k_find_flush_markers<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(d_in, n, d_list, d_count, cap);
+  count_launch();
+  return cudaGetLastError();
+}
+
+// ---- K12 (inflate_chunked.cuh): one stream by many chunks ----
+cudaError_t ck_launch_find(const uint8_t *in, uint32_t in_len, const unsigned long long *lo, const unsigned long long *hi,
+                           unsigned long long *cand, uint32_t n, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  k_inflate_find_blocks<<<n, 32, 0, s>>>(in, in_len, lo, hi, cand, n);
+  count_launch();
+  return cudaGetLastError();
+}
+cudaError_t ck_launch_chunks(const uint8_t *in, uint32_t in_len, const CkJob *jobs, uint32_t n, CkRes *res, uint16_t *pool,
+                             CkPage *pinfo, uint32_t *page_ctr, uint32_t n_pages, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  k_inflate_chunks<<<(n + 31) / 32, 32, 0, s>>>(in, in_len, jobs, n, res, pool, pinfo, page_ctr, n_pages);
+  count_launch();
+  return cudaGetLastError();
+}
+cudaError_t ck_launch_resolve(const CkChain *chain, uint32_t n_chain, const uint32_t *flat, const uint32_t *flat_chunk,
+                              uint32_t n_flat, const uint16_t *pool, uint8_t *out, unsigned long long lo_valid, uint32_t *bad,
+                              cudaStream_t s) {
+  if (n_chain == 0) return cudaSuccess;
+  k_inflate_windows<<<1, CK_WIN_THREADS, 0, s>>>(chain, n_chain, flat, pool, out, lo_valid, bad);
+  count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || n_flat == 0) return e;
+  k_inflate_emit<<<n_flat, 256, 0, s>>>(chain, flat, flat_chunk, pool, out, lo_valid, bad);
   count_launch();
   return cudaGetLastError();
 }

@@ -106,6 +106,7 @@ struct Ctl {
   uint32_t btype, bfinal, st_src, st_len;
   uint32_t hlit, hdist, maxl, maxd, sub_used, nlong_l, nlong_d;
   uint32_t nl, L, K, bm_stride, bm_off, p0;
+  uint32_t ck_off, arr_off;  // the lanes' checkpoint counts (0: none this block) and the per-lane result arrays, in the window
   uint32_t blk_end, blk_total;
   uint32_t x_state, x_olen, x_wofs;  // for the LZ77-only warps: 0 end, 1 nothing to do for this unit, 2 LZ77 over x_olen bytes
   uint32_t lz_next;                  // LZ77: the next bitmap word nobody has taken yet
@@ -136,6 +137,7 @@ static uint8_t *fp_emu_base = nullptr;
 #define FP_LDS32(a) (*reinterpret_cast<const uint32_t *>(fp_emu_base + (a)))
 #define FP_STS32(a, v) (*reinterpret_cast<uint32_t *>(fp_emu_base + (a)) = (v))
 #define FP_STS8(a, v) (*(fp_emu_base + (a)) = (uint8_t)(v))
+#define FP_STS16(a, v) (*reinterpret_cast<uint16_t *>(fp_emu_base + (a)) = (uint16_t)(v))
 #else
 #define FP_DEV __device__ __forceinline__
 #define FP_SPIN() ((void)0)
@@ -178,9 +180,13 @@ __device__ __forceinline__ uint32_t fp_lds32(uint32_t a) {
 }
 __device__ __forceinline__ void fp_sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void fp_sts8(uint32_t a, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void fp_sts16(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((unsigned short)v) : "memory");
+}
 #define FP_LDS32(a) fp_lds32(a)
 #define FP_STS32(a, v) fp_sts32((a), (v))
 #define FP_STS8(a, v) fp_sts8((a), (v))
+#define FP_STS16(a, v) fp_sts16((a), (v))
 #endif
 
 // FP_PROF builds (scripts/build_variant.sh prof -DFP_PROF): thread 0 adds the clocks between the barriers of a unit to
@@ -196,8 +202,8 @@ __device__ unsigned long long g_fp_prof[20];
       tl_ = t_;                                                             \
     }                                                                       \
   } while (0)
-// ... and every warp's lane 0 adds the clocks it WAITED at the barrier that ends pass A / A2 / A3 / C / LZ77 to
-// g_fp_prof[12 + k] (sum over the CTA's warps: 8 x the phase's clocks would mean everybody waited all the time)
+// ... and every warp's lane 0 adds the clocks it WAITED at the barrier that ends pass A / A2 / the false-start count / C /
+// LZ77 to g_fp_prof[12 + k] (sum over the CTA's warps: 8 x the phase's clocks would mean everybody waited all the time)
 #define FP_ARR() ta_ = clock64()
 #define FP_TICKW(k)                                                                      \
   do {                                                                                   \
@@ -265,17 +271,22 @@ FP_DEV uint32_t fp_lookup(uint32_t bits, bool dm, const uint32_t *lutl, const ui
 // updated by selects.  It only ever COMMITS ordinary symbols; whatever needs thought -- end of
 // block, an invalid code, the last 32 bits of the input, the place this lane has to stop at -- ends the loop BEFORE the
 // symbol is consumed, and the careful step of the calling pass decodes that symbol again with all its checks.
-//   MODE 0  pass A : count bytes, mark token boundaries in the lane's bitmap, stop at the end of the segment
+//   MODE 0  pass A : count bytes, mark token boundaries in the lane's bitmap, stop at the end of the segment; the first
+//                    boundary marked in a bitmap word also records the byte count there (its checkpoint)
 //   MODE 1  pass A2: count bytes, stop at a boundary the successor has marked too (or beyond its window)
-//   MODE 2  pass A3: count bytes, stop at `stop`
+//   MODE 2  false-start count: count bytes, stop at `stop`
 //   MODE 3  pass C : write bytes / match records into the window, stop at `stop`
 #ifdef FP_DEBUG
 static unsigned long fp_dbg_restarts = 0, fp_dbg_fastiters = 0;
+// false starts counted: from a checkpoint that is the meeting point / from a checkpoint before it / from the guessed
+// offset because the block has no checkpoints or the lane's count outgrew them
+static unsigned long fp_dbg_ck_exact = 0, fp_dbg_ck_walk = 0, fp_dbg_ck_full = 0;
 #endif
 struct FastCtx {
   uint32_t s_in, s_lutl, s_lutd, s_sub;  // shared addresses: staged input, the two root tables, the second level
   uint32_t end_bit, stop;         // bits of the unit; where this lane stops (a token boundary >= stop), NONE = never
   uint32_t org, K, s_row;         // MODE 0: my segment start / window / my bitmap row; MODE 1: the successor's
+  uint32_t s_ck;                  // MODE 0: my row of checkpoint counts (u16 per bitmap word), NONE = none this block
   uint32_t s_W;                   // MODE 3: shared address of output byte 0
   uint32_t *flags;                // MODE 3: match-start bitmap
 };
@@ -306,8 +317,9 @@ FP_DEV bool fp_fast(BR &br, bool &dm_io, uint32_t &pend_io, uint32_t &acc_io, ui
       if (MODE == 0) {
         const uint32_t rel = pos - c.org;
         if (rel < c.K) {
-          const uint32_t a = c.s_row + ((rel >> 5) << 2);
-          FP_STS32(a, FP_LDS32(a) | (1u << (rel & 31u)));
+          const uint32_t a = c.s_row + ((rel >> 5) << 2), old = FP_LDS32(a);
+          FP_STS32(a, old | (1u << (rel & 31u)));
+          if (old == 0u && c.s_ck != NONE) FP_STS16(c.s_ck + ((rel >> 5) << 1), acc);
         }
       }
       if (MODE == 1) {
@@ -599,8 +611,17 @@ FP_DEV void fp_plan_lanes(Ctl *ctl, uint32_t wofs) {
   ctl->nl = nl;
   ctl->L = nl > 1u ? L : 0u;
   ctl->K = nl > 1u ? K : 0u;
-  ctl->bm_stride = nl > 1u ? K / 32u + 1u : 0u;  // (+1: one spare word, and rows that do not all start in one bank)
-  ctl->bm_off = nl > 1u ? ((WIN + 16u - nl * (K / 32u + 1u) * 4u) & ~3u) : 0u;
+  const uint32_t bms = nl > 1u ? K / 32u + 1u : 0u;  // (+1: one spare word, and rows that do not all start in one bank)
+  ctl->bm_stride = bms;
+  ctl->bm_off = nl > 1u ? ((WIN + 16u - nl * bms * 4u) & ~3u) : 0u;
+  // Below the bitmaps, if the room holds them: the checkpoint counts (u16 per bitmap word) and the lanes' result arrays
+  // (tgt, pos, start).  The bitmaps then stay intact until the false starts are counted.  Otherwise -- late blocks of a
+  // unit whose output nearly fills the window -- the arrays take the dead bitmaps' place and every false start is decoded
+  // from its guessed offset.  (K is chosen as if there were no checkpoints: it decides which lanes meet.)
+  const uint32_t ckb = (nl * bms * 2u + 3u) & ~3u;
+  const bool ck = nl > 1u && nl * bms * 4u + ckb + nl * 12u <= room;
+  ctl->ck_off = ck ? ctl->bm_off - ckb : 0u;
+  ctl->arr_off = ck ? ctl->bm_off - ckb - nl * 12u : ctl->bm_off;
 }
 
 // ---------------- LZ77: matches copy shared -> shared ----------------
@@ -993,6 +1014,7 @@ k_inflate_fast(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__
   fc.s_lutl = FP_SA(lutl);
   fc.s_lutd = FP_SA(lutd);
   fc.s_sub = FP_SA(sub);
+  fc.s_ck = NONE;
   fc.flags = flags;
 
   if (tid >= (uint32_t)NT) {  // the LZ77-only warps (FP_XT): two CTA-wide barriers per unit, the pass in between
@@ -1199,8 +1221,10 @@ k_inflate_fast(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__
       const uint32_t nl = ctl->nl, L = ctl->L, K = ctl->K, bms = ctl->bm_stride, p0 = ctl->p0;
       const uint32_t maxl = ctl->maxl, maxd = ctl->maxd, olen0 = ctl->olen;
       uint32_t *const bm = reinterpret_cast<uint32_t *>(win + ctl->bm_off);
-      // per-lane results of the block: they take over the bitmaps' place once those are dead (one lane: the group counters')
-      uint32_t *const tgt_arr = nl > 1u ? bm : grp, *const pos_arr = tgt_arr + nl, *const start_arr = tgt_arr + 2u * nl;
+      uint16_t *const ck = ctl->ck_off != 0u ? reinterpret_cast<uint16_t *>(win + ctl->ck_off) : nullptr;
+      // per-lane results of the block (fp_plan_lanes places them; one lane: the group counters')
+      uint32_t *const tgt_arr = nl > 1u ? reinterpret_cast<uint32_t *>(win + ctl->arr_off) : grp, *const pos_arr = tgt_arr + nl,
+                     *const start_arr = tgt_arr + 2u * nl;
       const bool lane_on = tid < nl;
       const uint32_t myS = p0 + tid * L;
       const uint32_t segEnd = (tid + 1u < nl) ? myS + L : NONE;
@@ -1222,6 +1246,7 @@ k_inflate_fast(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__
         fc.stop = segEnd;
         fc.org = myS;
         fc.s_row = FP_SA(bm + tid * bms);
+        fc.s_ck = ck ? FP_SA(ck + tid * bms) : NONE;
       }
       // (the warp meets at every turn of these loops: a lane that leaves the bulk loop early must not run on by itself)
       while (__any_sync(FULL, state == 0)) {
@@ -1236,7 +1261,11 @@ k_inflate_fast(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__
               break;
             }
             const uint32_t rel = pos - myS;
-            if (rel < K) bm[tid * bms + (rel >> 5)] |= 1u << (rel & 31u);
+            if (rel < K) {
+              uint32_t &bw = bm[tid * bms + (rel >> 5)];
+              if (bw == 0u && ck) ck[tid * bms + (rel >> 5)] = (uint16_t)G;
+              bw |= 1u << (rel & 31u);
+            }
           }
           const int rem = (int)(end_bit - pos);
           const uint32_t bits = (uint32_t)br.buf;
@@ -1246,6 +1275,7 @@ k_inflate_fast(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__
           if (rem < 32) bad = bad || rem < (int)(dm ? maxd : maxl) || (int)(n + xb) > rem;
           if (bad || kind == K_EOB) {
             // a lane that dies while it still decodes from its guessed offset has lost nothing: guess again one bit on
+            // (its checkpoint counts need no clearing: a word's count is written again with the word's first new mark)
             if (tid > 0u && tokpos + 1u - myS < K / 2u) {
               for (uint32_t w = 0; w < bms; ++w) bm[tid * bms + w] = 0;
               sprime = tokpos + 1u;
@@ -1405,17 +1435,30 @@ k_inflate_fast(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__
       FP_DSYNC();
       FP_TICK(6);
       const uint32_t start = !valid ? 0u : tid == 0u ? p0 : start_arr[tid];
-      // ---------------- pass A3: bytes of my false start (my guessed offset .. where the true parse met me) ----------------
+      // ---------------- the bytes of my false start (my guessed offset .. where the true parse met me) ----------------
+      // `start` is one of my own marks, so the checkpoint of its bitmap word -- the word's first mark and my byte count
+      // there -- lies at or before it on my parse: at most 31 bits are decoded again.  Without checkpoints this block, or
+      // with a count too large for them, the whole false start is.
       uint32_t nbytes = 0;
       bool incons = false;
       {
         uint32_t f = 0, p3 = 0, t3 = sprime;
         bool d3 = false, go3 = valid && start != sprime;
+        const bool from_ck = go3 && ck && G <= 0xffffu;  // (counts only grow: then every checkpoint count kept all its bits)
+        if (from_ck) {
+          const uint32_t j = (start - myS) >> 5;
+          t3 = myS + j * 32u + (uint32_t)(__ffs((int)bm[tid * bms + j]) - 1);
+          f = ck[tid * bms + j];
+          go3 = t3 != start;
+        }
+#ifdef FP_DEBUG
+        if (valid && start != sprime) (!from_ck ? fp_dbg_ck_full : go3 ? fp_dbg_ck_walk : fp_dbg_ck_exact)++;
+#endif
         BR b3;
         b3.buf = 0;
         b3.cnt = 0;
         b3.wp = 0;
-        if (go3) br_seek(b3, in32, sprime);
+        if (go3) br_seek(b3, in32, t3);
         fc.stop = start;
         while (__any_sync(FULL, go3)) {
           if (go3) do {

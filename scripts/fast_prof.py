@@ -10,8 +10,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 import bench  # noqa: E402
 
-NAMES = ["store wait / loop top", "input wait", "header (thread 0)", "tables", "pass A", "pass A2", "chain walk", "pass A3 + scan",
-         "pass C", "end of blocks + next fetch", "LZ77", "store issue"]
+NAMES = ["store wait / loop top", "input wait", "header (thread 0)", "tables", "pass A", "pass A2", "chain walk",
+         "false-start count + scan", "pass C", "end of blocks + next fetch", "LZ77", "store issue"]
 
 
 def main():
@@ -60,7 +60,7 @@ def main():
     for i, name in enumerate(NAMES):
         print(f"  {name:28s} {buf[i] / k:9.0f}  {100.0 * buf[i] / tot:5.1f} %")
     print("  waited at the closing barrier, mean over the 8 warps (clocks per unit; share of the phase):")
-    for j, (name, ph) in enumerate([("pass A", 4), ("pass A2", 5), ("pass A3 + scan", 7), ("pass C", 8), ("LZ77", 10)]):
+    for j, (name, ph) in enumerate([("pass A", 4), ("pass A2", 5), ("false-start count + scan", 7), ("pass C", 8), ("LZ77", 10)]):
         print(f"  {name:28s} {buf[12 + j] / k / 8:9.0f}  {100.0 * buf[12 + j] / 8 / max(buf[ph], 1):5.1f} %")
 
 

@@ -2800,6 +2800,10 @@ extern "C" void b200z_debug_inflate_chunked_stats(unsigned long long out[6]) {
 extern "C" void b200z_debug_inflate_chunked_ms(double out[3]) {
   for (int k = 0; k < 3; ++k) out[k] = g_ck_ms[k];
 }
+// (test hook) cap on the blocks b200z_bzip2_encode sorts and codes in one batch (0: the built-in plan), so that inputs of a
+// few blocks run through several batches
+static uint32_t g_bz2e_max_batch = 0;
+extern "C" void b200z_debug_bzip2_encode_batch_set(unsigned max_batch) { g_bz2e_max_batch = max_batch; }
 
 extern "C" {
 
@@ -2899,7 +2903,8 @@ int b200z_bzip2_encode(const uint8_t *in, size_t in_len, uint8_t *out, size_t ou
   size_t free_b = 0, total_b = 0;
   CU(cudaMemGetInfo(&free_b, &total_b));
   const size_t budget = free_b + g.d_ws.cap > ((size_t)2 << 30) ? (free_b + g.d_ws.cap) / 2 : ((size_t)1 << 30);
-  const bz2e::Plan plan = bz2e::plan(in_len, budget < ((size_t)24 << 30) ? budget : ((size_t)24 << 30));
+  bz2e::Plan plan = bz2e::plan(in_len, budget < ((size_t)24 << 30) ? budget : ((size_t)24 << 30));
+  if (g_bz2e_max_batch && g_bz2e_max_batch < plan.batch) plan.batch = g_bz2e_max_batch;
   const size_t cap = align_up(bz2e::bound(in_len) + 64, 256);
   CU(g.d_out.reserve(cap));
   CU(g.d_ws.reserve(plan.ws_bytes));

@@ -292,13 +292,14 @@ struct OneResult {
 // `shared_output`: the stream is a gzip member -- everything already in g.d_out[0, out_pos) belongs to the same OutputStream
 // and is within reach of its back-references (InflateWs::hist)
 // ---------------------------------------------------------------------------------------------
-// K12: one stream decoded by many chunks (inflate_chunked.cuh, DESIGN.md "K12").  The stream's compressed input is
+// K12: large streams, each decoded by many chunks (inflate_chunked.cuh, DESIGN.md "K12").  A stream's compressed input is
 // worked through in regions that double from g_ck.thresh bytes: per region the block finder guesses a block start in
 // every chunk, all chunks decode at once, the chain is proven on the host from the region's exact start and the chunks
 // that started at a wrong guess are redone from their predecessor's end; then the windows are resolved and the region
 // is written to its final place.  The result is accepted only when the chain reaches a final block with every chunk
 // on it clean, no back-reference reaches before the allowed history and the output fits the cap; anything else leaves
-// the stream to the exact single-unit path, which gives every other result exactly.
+// the stream to the exact path, which gives every other result exactly.  A batch of streams (large ZIP members) moves
+// through these phases in lockstep, one launch per phase for all of them; a single stream is the batch of one.
 // ---------------------------------------------------------------------------------------------
 // Compressed bytes from which a stream takes K12, and the chunk size (0: a region's bytes over CK_TARGET, at least
 // CK_MIN_CHUNK).  Both are set by the benchmark's measurements (DESIGN.md "K12"); b200z_debug_inflate_chunked_set moves them
@@ -338,268 +339,382 @@ static size_t ck_carve(size_t &o, size_t bytes) {
   return at;
 }
 
-// Returns B200Z_OK with *accepted set when K12 produced the stream's result; an error code only for CUDA failures.
-static int run_chunked(const uint8_t *h_in, size_t pos, uint32_t il, size_t out_pos, uint32_t oc, uint32_t hist, OneResult *r,
-                       bool *accepted) {
-  *accepted = false;
-  for (auto &v : g_ck_stats) v = 0;
-  g_ck_stats[5] = 1;
-  CkTimer tm;
-  const uint8_t *in = (const uint8_t *)g.d_in.p + pos;
-  // the exact path's workspace for the same call: the pool is carved from it
-  const size_t ws = workspace_bytes(1, out_pos + oc);
-  CU(g.d_ws.reserve(ws));
-  const size_t max_ch = CK_TARGET + 8;
-  size_t o = 0;
-  const size_t o_lo = ck_carve(o, max_ch * 8), o_hi = ck_carve(o, max_ch * 8), o_cand = ck_carve(o, max_ch * 8);
-  const size_t o_jobs = ck_carve(o, max_ch * sizeof(CkJob)), o_res = ck_carve(o, max_ch * sizeof(CkRes));
-  const size_t o_chain = ck_carve(o, max_ch * sizeof(CkChain)), o_ctr = ck_carve(o, 16);
-  const size_t fixed = o;
-  // page records, the flat page list and the pages, plus the alignment the carving below may add (three times 256)
-  const size_t per_page = (size_t)CK_PAGE * 2 + sizeof(CkPage) + 8;
-  if (ws < fixed + 1024 + 8 * per_page) {  // (checked before the subtraction: a small cap gives a small workspace)
-    g_ck_stats[4] = 1;
-    return B200Z_OK;
+// One stream of a K12 batch, as the host sees it.
+struct CkIn {
+  const uint8_t *h_in;  // host copy of its compressed bytes (the stored-block checks below read a few of them)
+  size_t pos;           // its first compressed byte in g.d_in
+  uint32_t il;          // its compressed bytes
+  size_t out_pos;       // its first output byte in g.d_out
+  uint32_t oc;          // its output room
+  uint32_t hist;        // bytes in front of out_pos its back-references may reach
+  uint32_t n_pages;     // its share of the pool (ck_pages_for, not 0)
+};
+struct CkOut {
+  bool accepted = false;
+  OneResult r{};
+  unsigned long long stats[5] = {};  // regions, chunks, redo rounds, chunks merged, fell back
+};
+
+// g.d_ws for a batch of ns streams: the per-chunk records, the stream table and counters, then n_pages pages
+struct CkLayout {
+  size_t finds, cand, jobs, res, chain, chain_lo, streams, ctr, fixed, pinfo, flat, pool, bytes;
+  CkLayout(size_t ns, size_t n_pages) {
+    const size_t mc = ns * (CK_TARGET + 8);
+    size_t o = 0;
+    finds = ck_carve(o, mc * sizeof(CkFind));
+    cand = ck_carve(o, mc * 8);
+    jobs = ck_carve(o, mc * sizeof(CkJob));
+    res = ck_carve(o, mc * sizeof(CkRes));
+    chain = ck_carve(o, mc * sizeof(CkChain));
+    chain_lo = ck_carve(o, (ns + 1) * 4);
+    streams = ck_carve(o, ns * sizeof(CkStream));
+    ctr = ck_carve(o, ns * 8);  // page counters, then "reached too far" flags
+    fixed = o;
+    pinfo = ck_carve(o, n_pages * sizeof(CkPage));
+    flat = ck_carve(o, n_pages * 8);  // the flat page list, then the chain entry of each
+    pool = ck_carve(o, n_pages * (size_t)CK_PAGE * 2);
+    bytes = o;
   }
-  const size_t n_pages_sz = (ws - fixed - 1024) / per_page;
-  const uint32_t n_pages = (uint32_t)std::min<size_t>(n_pages_sz, 0xffffffu);
-  const size_t o_pinfo = ck_carve(o, (size_t)n_pages * sizeof(CkPage)), o_flat = ck_carve(o, (size_t)n_pages * 8);
-  const size_t o_pool = ck_carve(o, (size_t)n_pages * CK_PAGE * 2);
+};
+// a page: its symbols, its record and its two flat-list entries
+constexpr size_t CK_PER_PAGE = (size_t)CK_PAGE * 2 + sizeof(CkPage) + 8;
+
+// The pages of one stream's pool when it may use `ws` bytes -- the exact path's workspace for the same output, so that K12
+// never takes more device memory than the exact path would -- or 0 when that is too small to be worth carving.
+// (Checked before the subtraction: a small output room gives a small workspace.  The 1024 bytes cover the alignment of
+// the three page arrays.)
+static uint32_t ck_pages_for(size_t ws) {
+  const size_t fixed = CkLayout(1, 0).fixed;
+  if (ws < fixed + 1024 + 8 * CK_PER_PAGE) return 0;
+  return (uint32_t)std::min<size_t>((ws - fixed - 1024) / CK_PER_PAGE, 0xffffffu);
+}
+
+// Moves every stream of `in` through K12 in lockstep: per phase one launch for all the streams still live (the block
+// finder, the chunk decodes, each redo round, windows + emit).  Every acceptance and fallback rule is the single stream's,
+// applied per stream: a stream that falls back drops out and leaves the others running.  out[s].accepted: K12 produced
+// stream s's result (out[s].r); otherwise it is the exact path's to decode.  An error code only for CUDA failures.
+static int run_chunked(const std::vector<CkIn> &in, std::vector<CkOut> &out, double ms[3]) {
+  const size_t ns = in.size();
+  out.assign(ns, CkOut());
+  CkTimer tm;
+  size_t total_pages = 0;
+  for (const CkIn &c : in) total_pages += c.n_pages;
+  const CkLayout ly(ns, total_pages);
+  CU(g.d_ws.reserve(ly.bytes));
   uint8_t *w = (uint8_t *)g.d_ws.p;
-  auto *d_lo = (unsigned long long *)(w + o_lo), *d_hi = (unsigned long long *)(w + o_hi), *d_cand = (unsigned long long *)(w + o_cand);
-  auto *d_jobs = (CkJob *)(w + o_jobs);
-  auto *d_res = (CkRes *)(w + o_res);
-  auto *d_chain = (CkChain *)(w + o_chain);
-  auto *d_ctr = (uint32_t *)(w + o_ctr);
-  auto *d_pinfo = (CkPage *)(w + o_pinfo);
-  auto *d_flat = (uint32_t *)(w + o_flat);
-  auto *d_pool = (uint16_t *)(w + o_pool);
+  auto *d_finds = (CkFind *)(w + ly.finds);
+  auto *d_cand = (unsigned long long *)(w + ly.cand);
+  auto *d_jobs = (CkJob *)(w + ly.jobs);
+  auto *d_res = (CkRes *)(w + ly.res);
+  auto *d_chain = (CkChain *)(w + ly.chain);
+  auto *d_chain_lo = (uint32_t *)(w + ly.chain_lo);
+  auto *d_streams = (CkStream *)(w + ly.streams);
+  auto *d_ctr = (uint32_t *)(w + ly.ctr), *d_bad = d_ctr + ns;
+  auto *d_pinfo = (CkPage *)(w + ly.pinfo);
+  auto *d_flat = (uint32_t *)(w + ly.flat);
+  auto *d_pool = (uint16_t *)(w + ly.pool);
+  const uint8_t *d_in = (const uint8_t *)g.d_in.p;
   uint8_t *d_out = (uint8_t *)g.d_out.p;
-  const unsigned long long lo_valid = out_pos - hist;
-  const unsigned long long end_bits = 8ull * il;
+
+  struct St {  // a stream's progress
+    bool live = true, final_seen = false, proving = false;
+    unsigned long long bit0 = 0, end_bits = 0, pos_b = 0;  // the region's exact start; the input's end; the proven end
+    size_t emitted = 0, R = 0, rend = 0, span = 0, n = 0, find0 = 0, job0 = 0, total = 0;
+    std::vector<unsigned long long> S, cand;
+    std::vector<CkJob> jobs;
+    std::vector<CkRes> res;
+    std::vector<uint32_t> on_chain;
+  };
+  std::vector<St> st(ns);
+  std::vector<CkStream> tab(ns);
+  for (size_t s = 0, page0 = 0; s < ns; ++s) {
+    tab[s] = CkStream{(unsigned long long)in[s].pos, (unsigned long long)(in[s].out_pos - in[s].hist), in[s].il, (uint32_t)page0,
+                      in[s].n_pages, 0};
+    page0 += in[s].n_pages;
+    st[s].end_bits = 8ull * in[s].il;
+    st[s].R = g_ck.thresh;
+  }
+  CU(cudaMemcpyAsync(d_streams, tab.data(), ns * sizeof(CkStream), cudaMemcpyHostToDevice, g.stream));
+  auto fall = [&](size_t s) {
+    out[s].stats[4] = 1;
+    st[s].live = false;
+  };
   // A block that is not final starts at `e` with a stored header that reads the same LEN / NLEN as the one found at `c`:
   // bits e .. e + 2 are 000 and both reach the same byte boundary.
-  auto bit_at = [&](unsigned long long b) { return b < end_bits ? (h_in[b >> 3] >> (b & 7)) & 1u : 1u; };
-  auto stored_alike = [&](unsigned long long e, unsigned long long c) {
-    return ((e + 10) >> 3) == ((c + 10) >> 3) && bit_at(e) == 0 && bit_at(e + 1) == 0 && bit_at(e + 2) == 0;
+  auto bit_at = [&](size_t s, unsigned long long b) {
+    return b < st[s].end_bits ? (in[s].h_in[b >> 3] >> (b & 7)) & 1u : 1u;
   };
+  auto stored_alike = [&](size_t s, unsigned long long e, unsigned long long c) {
+    return ((e + 10) >> 3) == ((c + 10) >> 3) && bit_at(s, e) == 0 && bit_at(s, e + 1) == 0 && bit_at(s, e + 2) == 0;
+  };
+  for (size_t s = 0; s < ns; ++s)  // a stream that opens with a stored block: incompressible data, see below
+    if (bit_at(s, 1) == 0 && bit_at(s, 2) == 0) fall(s);
 
-  if (bit_at(1) == 0 && bit_at(2) == 0) {  // a stream that opens with a stored block: incompressible data, see below
-    g_ck_stats[4] = 1;
-    return B200Z_OK;
-  }
-  unsigned long long bit0 = 0;  // the region's exact start
-  size_t emitted = 0, R = g_ck.thresh;
-  std::vector<unsigned long long> S, lo, hi, cand;
-  std::vector<CkJob> jobs, redo;
-  std::vector<CkRes> res;
-  std::vector<CkPage> pinfo;
+  std::vector<CkFind> finds;
+  std::vector<unsigned long long> cand_all;
+  std::vector<CkJob> jobs_all;
+  std::vector<CkRes> res_all;
+  std::vector<std::pair<uint32_t, uint32_t>> redo_at;  // (stream, job) of each redone chunk
+  std::vector<CkPage> pinfo(total_pages);
   std::vector<CkChain> chain;
-  std::vector<uint32_t> flat, flat_chunk, on_chain;
+  std::vector<uint32_t> flat, flat_chunk, chain_lo, walks, ctr(ns), bad(ns), slot_to_chain;
   for (;;) {
-    g_ck_stats[0]++;
-    const size_t b0 = (size_t)(bit0 >> 3);
-    const size_t rend = std::min<size_t>(il, b0 + R);
-    const size_t span = rend - b0;
-    size_t C = g_ck.chunk ? g_ck.chunk : std::max<size_t>(CK_MIN_CHUNK, (span + CK_TARGET - 1) / CK_TARGET);
-    size_t n = std::max<size_t>(1, (span + C - 1) / C);
-    if (n > CK_TARGET) {
-      C = (span + CK_TARGET - 1) / CK_TARGET;
-      n = (span + C - 1) / C;
+    // ---- per live stream: its region, nominal chunk starts (chunk 0 starts at the proven bit0), and a block start guessed
+    // in every other chunk ----
+    finds.clear();
+    bool any = false;
+    for (size_t s = 0; s < ns; ++s) {
+      St &t = st[s];
+      if (!t.live) continue;
+      any = true;
+      out[s].stats[0]++;
+      const size_t il = in[s].il, b0 = (size_t)(t.bit0 >> 3);
+      t.rend = std::min<size_t>(il, b0 + t.R);
+      t.span = t.rend - b0;
+      size_t C = g_ck.chunk ? g_ck.chunk : std::max<size_t>(CK_MIN_CHUNK, (t.span + CK_TARGET - 1) / CK_TARGET);
+      size_t n = std::max<size_t>(1, (t.span + C - 1) / C);
+      if (n > CK_TARGET) {
+        C = (t.span + CK_TARGET - 1) / CK_TARGET;
+        n = (t.span + C - 1) / C;
+      }
+      t.n = n;
+      t.S.assign(n + 1, 0);
+      t.S[0] = t.bit0;
+      for (size_t k = 1; k < n; ++k) t.S[k] = 8ull * (b0 + k * C);
+      t.S[n] = t.rend == il ? ~0ull : 8ull * t.rend;
+      t.cand.assign(n, CK_NOCAND);
+      t.cand[0] = t.bit0;
+      t.find0 = finds.size();
+      for (size_t k = 1; k < n; ++k) finds.push_back(CkFind{t.S[k], std::min(t.S[k + 1], t.end_bits), (uint32_t)s, 0});
     }
-    // ---- nominal chunk starts, and a block start guessed in each (chunk 0 starts at the proven bit0) ----
-    S.assign(n + 1, 0);
-    S[0] = bit0;
-    for (size_t k = 1; k < n; ++k) S[k] = 8ull * (b0 + k * C);
-    S[n] = rend == il ? ~0ull : 8ull * rend;
-    cand.assign(n, CK_NOCAND);
-    cand[0] = bit0;
-    if (n > 1) {
-      lo.assign(S.begin() + 1, S.begin() + n);
-      hi.assign(S.begin() + 2, S.begin() + n + 1);
-      if (hi.back() > end_bits) hi.back() = end_bits;
-      CU(cudaMemcpyAsync(d_lo, lo.data(), lo.size() * 8, cudaMemcpyHostToDevice, g.stream));
-      CU(cudaMemcpyAsync(d_hi, hi.data(), hi.size() * 8, cudaMemcpyHostToDevice, g.stream));
+    if (!any) break;
+    if (!finds.empty()) {
+      cand_all.resize(finds.size());
+      CU(cudaMemcpyAsync(d_finds, finds.data(), finds.size() * sizeof(CkFind), cudaMemcpyHostToDevice, g.stream));
       tm.start();
-      CU(ck_launch_find(in, il, d_lo, d_hi, d_cand, (uint32_t)(n - 1), g.stream));
-      tm.stop(&g_ck_ms[0]);
-      CU(cudaMemcpyAsync(cand.data() + 1, d_cand, (n - 1) * 8, cudaMemcpyDeviceToHost, g.stream));
+      CU(ck_launch_find(d_in, d_streams, d_finds, d_cand, (uint32_t)finds.size(), g.stream));
+      tm.stop(&ms[0]);
+      CU(cudaMemcpyAsync(cand_all.data(), d_cand, finds.size() * 8, cudaMemcpyDeviceToHost, g.stream));
       CU(cudaStreamSynchronize(g.stream));
+      for (size_t s = 0; s < ns; ++s)
+        if (st[s].live) std::copy(cand_all.begin() + st[s].find0, cand_all.begin() + st[s].find0 + st[s].n - 1, st[s].cand.begin() + 1);
     }
     // ---- a chunk without a candidate is merged into its predecessor: jobs[i] covers up to the next kept start ----
-    jobs.clear();
-    for (size_t k = 0; k < n; ++k)
-      if (cand[k] != CK_NOCAND) jobs.push_back(CkJob{cand[k], 0, (uint32_t)jobs.size(), 0});
-    const size_t nj = jobs.size();
-    {
-      size_t i = 0;
-      for (size_t k = 0; k < n; ++k) {
-        if (cand[k] == CK_NOCAND) continue;
+    jobs_all.clear();
+    for (size_t s = 0; s < ns; ++s) {
+      St &t = st[s];
+      if (!t.live) continue;
+      const size_t n = t.n;
+      t.jobs.clear();
+      for (size_t k = 0; k < n; ++k)
+        if (t.cand[k] != CK_NOCAND) t.jobs.push_back(CkJob{t.cand[k], 0, (uint32_t)t.jobs.size(), 0, (uint16_t)s});
+      const size_t nj = t.jobs.size();
+      for (size_t k = 0, i = 0; k < n; ++k) {
+        if (t.cand[k] == CK_NOCAND) continue;
         size_t k2 = k + 1;
-        while (k2 < n && cand[k2] == CK_NOCAND) ++k2;
-        jobs[i++].stop_bit = S[k2];
+        while (k2 < n && t.cand[k2] == CK_NOCAND) ++k2;
+        t.jobs[i++].stop_bit = t.S[k2];
       }
-    }
-    g_ck_stats[1] += nj;
-    g_ck_stats[3] += n - nj;
-    // No block start found in a whole MiB (fixed-Huffman streams look like noise to the finder; stored blocks hold at most
-    // 64 KiB and zlib's dynamic ones far less): one lane would walk all of it, slower than the exact path's warp.
-    if (nj == 1 && span >= (1u << 20)) {
-      g_ck_stats[4] = 1;
-      return B200Z_OK;
-    }
-    // Mostly stored blocks (incompressible data): the exact path moves a stored block as one run of bytes, where a chunk
-    // lane copies it symbol by symbol; measured slower here (DESIGN.md "K12"), so such a stream stays on the exact path.
-    {
+      out[s].stats[1] += nj;
+      out[s].stats[3] += n - nj;
+      // No block start found in a whole MiB (fixed-Huffman streams look like noise to the finder; stored blocks hold at
+      // most 64 KiB and zlib's dynamic ones far less): one lane would walk all of it, slower than the exact path's warp.
+      if (nj == 1 && t.span >= (1u << 20)) {
+        fall(s);
+        continue;
+      }
+      // Mostly stored blocks (incompressible data): the exact path moves a stored block as one run of bytes, where a chunk
+      // lane copies it symbol by symbol; measured slower here (DESIGN.md "K12"), so such a stream stays on the exact path.
       size_t n_stored = 0;
-      for (const CkJob &jb : jobs) {
+      for (const CkJob &jb : t.jobs) {
         const size_t at = (size_t)((jb.start_bit + 10) >> 3);  // LEN of a stored block starting there
-        n_stored += bit_at(jb.start_bit + 1) == 0 && bit_at(jb.start_bit + 2) == 0 && at + 2 <= il &&
-                    (h_in[at] | (h_in[at + 1] << 8)) >= 1024;  // (flush markers are empty stored blocks)
+        n_stored += bit_at(s, jb.start_bit + 1) == 0 && bit_at(s, jb.start_bit + 2) == 0 && at + 2 <= in[s].il &&
+                    (in[s].h_in[at] | (in[s].h_in[at + 1] << 8)) >= 1024;  // (flush markers are empty stored blocks)
       }
       if (nj >= 8 && 2 * n_stored > nj) {
-        g_ck_stats[4] = 1;
-        return B200Z_OK;
+        fall(s);
+        continue;
       }
+      t.job0 = jobs_all.size();
+      jobs_all.insert(jobs_all.end(), t.jobs.begin(), t.jobs.end());
     }
-    CU(cudaMemsetAsync(d_ctr, 0, 4, g.stream));
-    CU(cudaMemcpyAsync(d_jobs, jobs.data(), nj * sizeof(CkJob), cudaMemcpyHostToDevice, g.stream));
+    if (jobs_all.empty()) continue;
+    CU(cudaMemsetAsync(d_ctr, 0, ns * 4, g.stream));
+    CU(cudaMemcpyAsync(d_jobs, jobs_all.data(), jobs_all.size() * sizeof(CkJob), cudaMemcpyHostToDevice, g.stream));
     tm.start();
-    CU(ck_launch_chunks(in, il, d_jobs, (uint32_t)nj, d_res, d_pool, d_pinfo, d_ctr, n_pages, g.stream));
-    tm.stop(&g_ck_ms[1]);
-    res.resize(nj);
-    CU(cudaMemcpyAsync(res.data(), d_res, nj * sizeof(CkRes), cudaMemcpyDeviceToHost, g.stream));
+    CU(ck_launch_chunks(d_in, d_streams, d_jobs, (uint32_t)jobs_all.size(), d_res, d_pool, d_pinfo, d_ctr, g.stream));
+    tm.stop(&ms[1]);
+    res_all.resize(jobs_all.size());
+    CU(cudaMemcpyAsync(res_all.data(), d_res, res_all.size() * sizeof(CkRes), cudaMemcpyDeviceToHost, g.stream));
     CU(cudaStreamSynchronize(g.stream));
-    // ---- prove the chain from bit0; redo what started at a wrong guess ----
-    bool final_seen = false;
-    unsigned long long pos_b = bit0;
-    on_chain.clear();
+    for (size_t s = 0; s < ns; ++s)
+      if (st[s].live) {
+        st[s].res.assign(res_all.begin() + st[s].job0, res_all.begin() + st[s].job0 + st[s].jobs.size());
+        st[s].proving = true;
+      }
+    // ---- prove every chain from its bit0; redo what started at a wrong guess (all streams' redos in one launch) ----
     for (int round = 0;; ++round) {
-      pos_b = bit0;
-      on_chain.clear();
-      final_seen = false;
-      size_t bad_at = nj;
-      for (size_t i = 0; i < nj; ++i) {
-        if (i > 0 && pos_b >= jobs[i].stop_bit) continue;  // its whole slice lies inside its predecessor's last block
-        if (jobs[i].start_bit != pos_b && res[i].first_stored && stored_alike(pos_b, jobs[i].start_bit))
-          jobs[i].start_bit = pos_b;  // the same stored block read from its true header: the same result
-        if (jobs[i].start_bit != pos_b) {
-          bad_at = i;
-          break;
+      jobs_all.clear();
+      redo_at.clear();
+      for (size_t s = 0; s < ns; ++s) {
+        St &t = st[s];
+        if (!t.live || !t.proving) continue;
+        const size_t nj = t.jobs.size();
+        std::vector<CkJob> &jobs = t.jobs;
+        std::vector<CkRes> &res = t.res;
+        t.pos_b = t.bit0;
+        t.on_chain.clear();
+        t.final_seen = false;
+        size_t bad_at = nj;
+        bool failed = false;
+        for (size_t i = 0; i < nj; ++i) {
+          if (i > 0 && t.pos_b >= jobs[i].stop_bit) continue;  // its whole slice lies inside its predecessor's last block
+          if (jobs[i].start_bit != t.pos_b && res[i].first_stored && stored_alike(s, t.pos_b, jobs[i].start_bit))
+            jobs[i].start_bit = t.pos_b;  // the same stored block read from its true header: the same result
+          if (jobs[i].start_bit != t.pos_b) {
+            bad_at = i;
+            break;
+          }
+          const int cs = res[i].status;
+          if (cs != CK_BOUNDARY && cs != CK_FINAL) {  // the exact step fails here too (or the stream's pages ran out)
+            failed = true;
+            break;
+          }
+          t.on_chain.push_back((uint32_t)i);
+          t.pos_b = res[i].end_bit;
+          if (cs == CK_FINAL) {
+            t.final_seen = true;
+            break;
+          }
         }
-        const int st = res[i].status;
-        if (st != CK_BOUNDARY && st != CK_FINAL) {  // the exact step fails here too (or the pool ran out)
-          g_ck_stats[4] = 1;
-          return B200Z_OK;
+        if (failed || (bad_at != nj && round >= CK_MAX_ROUNDS)) {
+          fall(s);
+          continue;
         }
-        on_chain.push_back((uint32_t)i);
-        pos_b = res[i].end_bit;
-        if (st == CK_FINAL) {
-          final_seen = true;
-          break;
+        if (bad_at == nj) {
+          t.proving = false;
+          continue;
         }
+        // Redo the first unproven chunk from the proven end and, together with it, every later chunk that does not start
+        // where its predecessor's last attempt ended (from that end: usually right, and proven or redone next round).
+        unsigned long long prev_end = t.pos_b;
+        for (size_t i = bad_at; i < nj; ++i) {
+          if (prev_end >= jobs[i].stop_bit) continue;  // empty: the end carries over
+          const bool mism = jobs[i].start_bit != prev_end && !(res[i].first_stored && stored_alike(s, prev_end, jobs[i].start_bit));
+          if (mism) {
+            jobs[i].start_bit = prev_end;
+            jobs[i].gen++;
+            jobs_all.push_back(jobs[i]);
+            redo_at.emplace_back((uint32_t)s, (uint32_t)i);
+          }
+          if (res[i].status != CK_BOUNDARY) break;
+          prev_end = res[i].end_bit;
+        }
+        out[s].stats[2]++;
       }
-      if (bad_at == nj) break;
-      if (round >= CK_MAX_ROUNDS) {
-        g_ck_stats[4] = 1;
-        return B200Z_OK;
-      }
-      // Redo the first unproven chunk from the proven end and, together with it, every later chunk that does not start
-      // where its predecessor's last attempt ended (from that end: usually right, and proven or redone next round).
-      redo.clear();
-      std::vector<size_t> redo_idx;
-      unsigned long long prev_end = pos_b;
-      for (size_t i = bad_at; i < nj; ++i) {
-        if (prev_end >= jobs[i].stop_bit) continue;  // empty: the end carries over
-        const bool mism = jobs[i].start_bit != prev_end &&
-                          !(res[i].first_stored && stored_alike(prev_end, jobs[i].start_bit));
-        if (mism) {
-          jobs[i].start_bit = prev_end;
-          jobs[i].gen++;
-          redo.push_back(jobs[i]);
-          redo_idx.push_back(i);
-        }
-        if (res[i].status != CK_BOUNDARY) break;
-        prev_end = res[i].end_bit;
-      }
-      g_ck_stats[2]++;
-      CU(cudaMemcpyAsync(d_jobs, redo.data(), redo.size() * sizeof(CkJob), cudaMemcpyHostToDevice, g.stream));
+      if (jobs_all.empty()) break;
+      CU(cudaMemcpyAsync(d_jobs, jobs_all.data(), jobs_all.size() * sizeof(CkJob), cudaMemcpyHostToDevice, g.stream));
       tm.start();
-      CU(ck_launch_chunks(in, il, d_jobs, (uint32_t)redo.size(), d_res, d_pool, d_pinfo, d_ctr, n_pages, g.stream));
-      tm.stop(&g_ck_ms[1]);
-      std::vector<CkRes> rr(redo.size());
-      CU(cudaMemcpyAsync(rr.data(), d_res, rr.size() * sizeof(CkRes), cudaMemcpyDeviceToHost, g.stream));
+      CU(ck_launch_chunks(d_in, d_streams, d_jobs, (uint32_t)jobs_all.size(), d_res, d_pool, d_pinfo, d_ctr, g.stream));
+      tm.stop(&ms[1]);
+      res_all.resize(jobs_all.size());
+      CU(cudaMemcpyAsync(res_all.data(), d_res, res_all.size() * sizeof(CkRes), cudaMemcpyDeviceToHost, g.stream));
       CU(cudaStreamSynchronize(g.stream));
-      for (size_t q = 0; q < redo.size(); ++q) res[redo_idx[q]] = rr[q];
+      for (size_t q = 0; q < redo_at.size(); ++q) st[redo_at[q].first].res[redo_at[q].second] = res_all[q];
     }
-    if (!final_seen && rend == il) {  // the input ends without a final block: the exact step's EOS / STOP
-      g_ck_stats[4] = 1;
-      return B200Z_OK;
-    }
-    // ---- output offsets, the chain's pages in order, then windows and bytes ----
-    uint32_t pages_used = 0;
-    CU(cudaMemcpyAsync(&pages_used, d_ctr, 4, cudaMemcpyDeviceToHost, g.stream));
+    for (size_t s = 0; s < ns; ++s)  // the input ends without a final block: the exact step's EOS / STOP
+      if (st[s].live && !st[s].final_seen && st[s].rend == in[s].il) fall(s);
+    // ---- per stream: output offsets and its chain's pages in order; then windows and bytes for all of them ----
+    CU(cudaMemcpyAsync(ctr.data(), d_ctr, ns * 4, cudaMemcpyDeviceToHost, g.stream));
     CU(cudaStreamSynchronize(g.stream));
-    pages_used = std::min(pages_used, n_pages);
-    pinfo.resize(pages_used);
-    if (pages_used) CU(cudaMemcpyAsync(pinfo.data(), d_pinfo, pages_used * sizeof(CkPage), cudaMemcpyDeviceToHost, g.stream));
+    for (size_t s = 0; s < ns; ++s) {
+      ctr[s] = std::min(ctr[s], in[s].n_pages);
+      if (st[s].live && ctr[s])
+        CU(cudaMemcpyAsync(pinfo.data() + tab[s].page0, d_pinfo + tab[s].page0, ctr[s] * sizeof(CkPage), cudaMemcpyDeviceToHost,
+                           g.stream));
+    }
     CU(cudaStreamSynchronize(g.stream));
     chain.clear();
-    std::vector<uint32_t> slot_to_chain(nj, 0xffffffffu);
-    size_t total = 0, nflat = 0;
-    for (uint32_t i : on_chain) {
-      slot_to_chain[i] = (uint32_t)chain.size();
-      chain.push_back(CkChain{(unsigned long long)(out_pos + emitted + total), res[i].nsym, (uint32_t)nflat});
-      total += res[i].nsym;
-      nflat += (res[i].nsym + CK_PAGE - 1) / CK_PAGE;
-    }
-    if (emitted + total > oc) {  // the exact path's NOSPC
-      g_ck_stats[4] = 1;
-      return B200Z_OK;
-    }
-    flat.assign(nflat, 0xffffffffu);
-    flat_chunk.assign(nflat, 0);
-    for (uint32_t p = 0; p < pages_used; ++p) {
-      const CkPage &pi = pinfo[p];
-      if (pi.slot >= nj || slot_to_chain[pi.slot] == 0xffffffffu || pi.gen != jobs[pi.slot].gen) continue;
-      const CkChain &c = chain[slot_to_chain[pi.slot]];
-      if ((size_t)pi.seq * CK_PAGE >= c.nsym) continue;
-      flat[c.page0 + pi.seq] = p;
-      flat_chunk[c.page0 + pi.seq] = slot_to_chain[pi.slot];
-    }
-    for (uint32_t f : flat)
-      if (f == 0xffffffffu) {  // (cannot happen: every symbol of a clean chunk is on a page)
-        g_ck_stats[4] = 1;
-        return B200Z_OK;
+    flat.clear();
+    flat_chunk.clear();
+    chain_lo.clear();
+    walks.clear();
+    for (size_t s = 0; s < ns; ++s) {
+      St &t = st[s];
+      if (!t.live) continue;
+      const size_t nj = t.jobs.size(), chain0 = chain.size(), flat0 = flat.size();
+      slot_to_chain.assign(nj, 0xffffffffu);
+      size_t total = 0, nflat = flat0;
+      for (uint32_t i : t.on_chain) {
+        slot_to_chain[i] = (uint32_t)chain.size();
+        chain.push_back(CkChain{(unsigned long long)(in[s].out_pos + t.emitted + total), t.res[i].nsym, (uint32_t)nflat, (uint32_t)s, 0});
+        total += t.res[i].nsym;
+        nflat += (t.res[i].nsym + CK_PAGE - 1) / CK_PAGE;
       }
-    if (!chain.empty()) {
+      bool ok = t.emitted + total <= in[s].oc;  // else the exact path's NOSPC
+      if (ok) {
+        flat.resize(nflat, 0xffffffffu);
+        flat_chunk.resize(nflat, 0);
+        for (uint32_t p = 0; p < ctr[s]; ++p) {
+          const CkPage &pi = pinfo[tab[s].page0 + p];
+          if (pi.slot >= nj || slot_to_chain[pi.slot] == 0xffffffffu || pi.gen != t.jobs[pi.slot].gen) continue;
+          const CkChain &c = chain[slot_to_chain[pi.slot]];
+          if ((size_t)pi.seq * CK_PAGE >= c.nsym) continue;
+          flat[c.page0 + pi.seq] = tab[s].page0 + p;
+          flat_chunk[c.page0 + pi.seq] = slot_to_chain[pi.slot];
+        }
+        for (size_t f = flat0; f < nflat && ok; ++f) ok = flat[f] != 0xffffffffu;  // (cannot fail: every symbol of a clean chunk is on a page)
+      }
+      if (!ok) {
+        chain.resize(chain0);
+        flat.resize(flat0);
+        flat_chunk.resize(flat0);
+        fall(s);
+        continue;
+      }
+      t.total = total;
+      if (chain.size() > chain0) {
+        chain_lo.push_back((uint32_t)chain0);
+        walks.push_back((uint32_t)s);
+      }
+    }
+    chain_lo.push_back((uint32_t)chain.size());
+    std::fill(bad.begin(), bad.end(), 0u);
+    if (!walks.empty()) {
+      const size_t nflat = flat.size();
       CU(cudaMemcpyAsync(d_chain, chain.data(), chain.size() * sizeof(CkChain), cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemcpyAsync(d_chain_lo, chain_lo.data(), chain_lo.size() * 4, cudaMemcpyHostToDevice, g.stream));
       CU(cudaMemcpyAsync(d_flat, flat.data(), nflat * 4, cudaMemcpyHostToDevice, g.stream));
       CU(cudaMemcpyAsync(d_flat + nflat, flat_chunk.data(), nflat * 4, cudaMemcpyHostToDevice, g.stream));
-      CU(cudaMemsetAsync(d_ctr + 1, 0, 4, g.stream));
+      CU(cudaMemsetAsync(d_bad, 0, ns * 4, g.stream));
       tm.start();
-      CU(ck_launch_resolve(d_chain, (uint32_t)chain.size(), d_flat, d_flat + nflat, (uint32_t)nflat, d_pool, d_out, lo_valid,
-                           d_ctr + 1, g.stream));
-      tm.stop(&g_ck_ms[2]);
-      uint32_t bad = 0;
-      CU(cudaMemcpyAsync(&bad, d_ctr + 1, 4, cudaMemcpyDeviceToHost, g.stream));
+      CU(ck_launch_resolve(d_chain, d_chain_lo, (uint32_t)walks.size(), d_flat, d_flat + nflat, (uint32_t)nflat, d_pool, d_out,
+                           d_streams, d_bad, g.stream));
+      tm.stop(&ms[2]);
+      CU(cudaMemcpyAsync(bad.data(), d_bad, ns * 4, cudaMemcpyDeviceToHost, g.stream));
       CU(cudaStreamSynchronize(g.stream));
-      if (bad) {  // a back-reference before the allowed history: the exact path's RANGE
-        g_ck_stats[4] = 1;
-        return B200Z_OK;
+    }
+    for (size_t s = 0; s < ns; ++s) {
+      St &t = st[s];
+      if (!t.live) continue;
+      if (bad[s]) {  // a back-reference before the allowed history: the exact path's RANGE
+        fall(s);
+        continue;
       }
+      t.emitted += t.total;
+      if (t.final_seen) {
+        out[s].r.out_len = (uint32_t)t.emitted;
+        out[s].r.in_used = (uint32_t)((t.pos_b + 7) >> 3);
+        out[s].r.status = B200Z_U_DONE;
+        out[s].accepted = true;
+        t.live = false;
+        continue;
+      }
+      t.bit0 = t.pos_b;
+      t.R *= 2;
     }
-    emitted += total;
-    if (final_seen) {
-      r->out_len = (uint32_t)emitted;
-      r->in_used = (uint32_t)((pos_b + 7) >> 3);
-      r->status = B200Z_U_DONE;
-      *accepted = true;
-      return B200Z_OK;
-    }
-    bit0 = pos_b;
-    R *= 2;
   }
+  return B200Z_OK;
 }
 
 // `try_chunked`: K12 may take the stream (the caller knows nothing that makes it pointless)
@@ -617,9 +732,22 @@ static int run_one_staged(const uint8_t *h_in, size_t pos, size_t in_total, size
   for (auto &v : g_ck_stats) v = 0;
   for (auto &v : g_ck_ms) v = 0;
   if (try_chunked && il >= g_ck.thresh) {
-    bool accepted = false;
-    int rc = run_chunked(h_in + pos, pos, il, out_pos, oc, hist, r, &accepted);
-    if (rc || accepted) return rc;
+    // the exact path's workspace for the same call: the pool is carved from it
+    const size_t ws = workspace_bytes(1, out_pos + oc);
+    CU(g.d_ws.reserve(ws));
+    const uint32_t n_pages = ck_pages_for(ws);
+    g_ck_stats[4] = g_ck_stats[5] = 1;
+    if (n_pages) {
+      const std::vector<CkIn> one{CkIn{h_in + pos, pos, il, out_pos, oc, hist, n_pages}};
+      std::vector<CkOut> res;
+      const int rc = run_chunked(one, res, g_ck_ms);
+      if (rc) return rc;
+      for (int k = 0; k < 5; ++k) g_ck_stats[k] = res[0].stats[k];
+      if (res[0].accepted) {
+        *r = res[0].r;
+        return B200Z_OK;
+      }
+    }
   }
   return run_batch_on_staged(&io, &il, &oo, &oc, &r->out_len, &r->status, &r->in_used, 1, out_pos + oc, false, hist);
 }
@@ -2219,8 +2347,99 @@ extern "C" int b200z_zip_comment(const uint8_t *z, size_t len, uint64_t *off, ui
 // the entries handed to zip_extract_core point there.
 struct ZipPlain {
   size_t staged;                                // bytes of g.d_in in use: the archive, then the plaintext area
+  size_t archive_len;                           // of which the archive (the bytes the host holds)
   const std::vector<const uint8_t *> *bz_src;   // per member: host copy of a decrypted bzip2 member, or null
 };
+
+// (test hooks) last b200z_zip_extract call's K12 batch: members offered, accepted, fell back, redo rounds, batches; kernel
+// times as g_ck_ms.  Caps on the streams of one batch and on each stream's pool pages (0: none, the built-in share).
+static unsigned long long g_zck_stats[5];
+static double g_zck_ms[3];
+static uint32_t g_zck_max_streams = 0, g_zck_max_pages = 0;
+
+// K12 for the large ZIP members (zip_extract_core): every unit that is a whole deflate member of g_ck.thresh compressed
+// bytes or more is decoded by K12 from exactly the input view its unit has, straight to its place in the output.  All
+// of them go through one K12 batch, or several when their pools do not fit: each member's pool is what its exact-path
+// workspace would be (ck_pages_for), and a batch takes at most the buffer K12 already has plus half the free device
+// memory.  Accepted members leave the unit list (their out_len is set here, their status stays B200Z_U_DONE); a member
+// K12 declines stays in the list at its place and the exact path decodes it as if K12 had never run.
+static int zip_chunked(const uint8_t *z, size_t len, const b200z_zip_entry *entries, const ZipPlain *pl,
+                       std::vector<uint64_t> &u_in_off, std::vector<uint32_t> &u_in_len, std::vector<uint64_t> &u_out_off,
+                       std::vector<uint32_t> &u_cap, std::vector<uint32_t> &u_idx, uint64_t *out_len) {
+  const size_t host_len = pl ? pl->archive_len : len;
+  std::vector<size_t> big;
+  for (size_t k = 0; k < u_idx.size(); ++k)  // (a split member's pieces carry the 0x80000000 mark or start behind data_off)
+    if (!(u_idx[k] & 0x80000000u) && u_in_off[k] == entries[u_idx[k]].data_off && u_in_len[k] >= g_ck.thresh) big.push_back(k);
+  if (big.empty()) return B200Z_OK;
+  size_t budget = g.d_ws.cap, free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) budget += free_b / 2;
+  std::vector<char> taken(u_idx.size(), 0);
+  std::vector<std::vector<uint8_t>> h_plain;  // host copies of decrypted members (their bytes live on the device only)
+  std::vector<CkIn> batch;
+  std::vector<size_t> at;
+  std::vector<CkOut> res;
+  for (size_t b = 0; b < big.size();) {
+    batch.clear();
+    at.clear();
+    h_plain.clear();
+    size_t pages = 0;
+    for (; b < big.size(); ++b) {
+      const size_t k = big[b];
+      uint32_t np = ck_pages_for(workspace_bytes(1, u_cap[k]));
+      if (g_zck_max_pages) np = std::min(np, g_zck_max_pages);
+      if (!batch.empty() && ((g_zck_max_streams && batch.size() >= g_zck_max_streams) ||
+                             CkLayout(batch.size() + 1, pages + np).bytes > budget))
+        break;
+      if (np == 0 || CkLayout(1, np).bytes > budget) {  // no pool, or not even on its own: left to the exact path
+        g_zck_stats[0]++;
+        g_zck_stats[2]++;
+        continue;
+      }
+      const uint8_t *h = z + u_in_off[k];
+      if (u_in_off[k] + u_in_len[k] > host_len) {
+        h_plain.emplace_back(u_in_len[k]);
+        CU(cudaMemcpyAsync(h_plain.back().data(), (const uint8_t *)g.d_in.p + u_in_off[k], u_in_len[k], cudaMemcpyDeviceToHost,
+                           g.stream));
+        h = h_plain.back().data();
+      }
+      batch.push_back(CkIn{h, (size_t)u_in_off[k], u_in_len[k], (size_t)u_out_off[k], u_cap[k], 0, np});
+      at.push_back(k);
+      pages += np;
+    }
+    if (batch.empty()) continue;
+    CU(cudaStreamSynchronize(g.stream));
+    const int rc = run_chunked(batch, res, g_zck_ms);
+    if (rc) return rc;
+    g_zck_stats[4]++;
+    for (size_t q = 0; q < batch.size(); ++q) {
+      g_zck_stats[0]++;
+      g_zck_stats[3] += res[q].stats[2];
+      if (!res[q].accepted) {
+        g_zck_stats[2]++;
+        continue;
+      }
+      g_zck_stats[1]++;
+      out_len[u_idx[at[q]]] = res[q].r.out_len;
+      taken[at[q]] = 1;
+    }
+  }
+  size_t m = 0;
+  for (size_t k = 0; k < u_idx.size(); ++k) {
+    if (taken[k]) continue;
+    u_in_off[m] = u_in_off[k];
+    u_in_len[m] = u_in_len[k];
+    u_out_off[m] = u_out_off[k];
+    u_cap[m] = u_cap[k];
+    u_idx[m] = u_idx[k];
+    m++;
+  }
+  u_in_off.resize(m);
+  u_in_len.resize(m);
+  u_out_off.resize(m);
+  u_cap.resize(m);
+  u_idx.resize(m);
+  return B200Z_OK;
+}
 
 // ZipFile.getStream for all members (g.mu held).  pl == nullptr: the archive is not staged yet and `len` is its size;
 // otherwise `len` = pl->staged and everything is in g.d_in already.
@@ -2378,6 +2597,12 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
         }
       }
     }
+  }
+  for (auto &v : g_zck_stats) v = 0;
+  for (auto &v : g_zck_ms) v = 0;
+  if (!u_idx.empty()) {
+    rc = zip_chunked(z, len, entries, pl, u_in_off, u_in_len, u_out_off, u_cap, u_idx, out_len);
+    if (rc) return rc;
   }
   size_t early_to = (size_t)lo;  // output bytes [lo, early_to) are on their way to the host already (copy stream)
   if (!u_idx.empty()) {
@@ -2672,7 +2897,7 @@ static int zip_extract_crypt(const uint8_t *z, size_t len, const b200z_zip_entry
   }
   if (!bz_keep.empty()) CU(cudaStreamSynchronize(g.stream));
   // 6. everything else sees the decrypted members as ranges of the staged buffer
-  const ZipPlain pl{staged, &bz_src};
+  const ZipPlain pl{staged, len, &bz_src};
   int rc = zip_extract_core(z, staged, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, &pl);
   if (rc) {
     cudaStreamSynchronize(s_mac);
@@ -2799,6 +3024,18 @@ extern "C" void b200z_debug_inflate_chunked_stats(unsigned long long out[6]) {
 // (test hook) the last single-stream call's K12 kernel times in ms (CUDA events): finder, chunk decodes, windows + emit
 extern "C" void b200z_debug_inflate_chunked_ms(double out[3]) {
   for (int k = 0; k < 3; ++k) out[k] = g_ck_ms[k];
+}
+// (test hooks) K12 for ZIP members (zip_chunked): caps on the members of one K12 batch and on each member's pool pages
+// (0 each: none, the built-in share), and the last b200z_zip_extract call's statistics -- members offered, accepted,
+// fell back, redo rounds, batches -- and kernel times in ms (finder, chunk decodes, windows + emit).  The threshold and
+// the chunk size are b200z_debug_inflate_chunked_set's.
+extern "C" void b200z_debug_zip_chunked_set(unsigned max_streams, unsigned max_pages) {
+  g_zck_max_streams = max_streams;
+  g_zck_max_pages = max_pages;
+}
+extern "C" void b200z_debug_zip_chunked_stats(unsigned long long out[5], double ms[3]) {
+  for (int k = 0; k < 5; ++k) out[k] = g_zck_stats[k];
+  for (int k = 0; k < 3; ++k) ms[k] = g_zck_ms[k];
 }
 // (test hook) cap on the blocks b200z_bzip2_encode sorts and codes in one batch (0: the built-in plan), so that inputs of a
 // few blocks run through several batches

@@ -58,14 +58,15 @@ struct InflateBatch {
 };
 
 cudaError_t launch_inflate(const InflateBatch &b, cudaStream_t stream);
-// K12 (inflate_chunked.cuh)
-cudaError_t ck_launch_find(const uint8_t *in, uint32_t in_len, const unsigned long long *lo, const unsigned long long *hi,
-                           unsigned long long *cand, uint32_t n, cudaStream_t s);
-cudaError_t ck_launch_chunks(const uint8_t *in, uint32_t in_len, const CkJob *jobs, uint32_t n, CkRes *res, uint16_t *pool,
-                             CkPage *pinfo, uint32_t *page_ctr, uint32_t n_pages, cudaStream_t s);
-cudaError_t ck_launch_resolve(const CkChain *chain, uint32_t n_chain, const uint32_t *flat, const uint32_t *flat_chunk,
-                              uint32_t n_flat, const uint16_t *pool, uint8_t *out, unsigned long long lo_valid, uint32_t *bad,
-                              cudaStream_t s);
+// K12 (inflate_chunked.cuh) over a batch of streams; `streams` is the device copy of the batch's stream table
+cudaError_t ck_launch_find(const uint8_t *in_base, const CkStream *streams, const CkFind *finds, unsigned long long *cand,
+                           uint32_t n, cudaStream_t s);
+cudaError_t ck_launch_chunks(const uint8_t *in_base, const CkStream *streams, const CkJob *jobs, uint32_t n, CkRes *res,
+                             uint16_t *pool, CkPage *pinfo, uint32_t *page_ctr, cudaStream_t s);
+// windows: one CTA per chain walk chain[chain_lo[w] .. chain_lo[w + 1]); then emit over the n_flat pages of all of them
+cudaError_t ck_launch_resolve(const CkChain *chain, const uint32_t *chain_lo, uint32_t n_walks, const uint32_t *flat,
+                              const uint32_t *flat_chunk, uint32_t n_flat, const uint16_t *pool, uint8_t *out,
+                              const CkStream *streams, uint32_t *bad, cudaStream_t s);
 cudaError_t launch_find_markers(const uint8_t *d_in, size_t n, unsigned long long *d_list, uint32_t *d_count, uint32_t cap,
                                 cudaStream_t stream);
 

@@ -1,11 +1,13 @@
-// inflate_chunked.cuh -- K12: one large raw DEFLATE stream decoded by many chunks at once (included by inflate_kernels.cu).
+// inflate_chunked.cuh -- K12: large raw DEFLATE streams, each decoded by many chunks at once (included by inflate_kernels.cu).
 //
 // A chunk starts at a block boundary guessed inside its slice of the compressed stream and decodes without the 32 KiB of
 // output in front of it: its output is 16-bit SYMBOLS, a value < 256 being a byte and 0x8000 | w byte w (0..32767) of the
 // window in front of the chunk (a match that copies from such a place copies the marker).  The host proves the chain of
 // chunks from the stream's true start and redoes the chunks that started at a wrong guess (b200z_api.cu:
 // run_chunked); then k_inflate_windows resolves the last 32 KiB of every chunk in chunk order, straight into the
-// output buffer, and k_inflate_emit translates every page of symbols in parallel.  DESIGN.md "K12".
+// output buffer, and k_inflate_emit translates every page of symbols in parallel.  Every kernel works on a batch of
+// streams (CkStream): a chunk, a job or a chain entry names its stream, and each stream has its own input, page range and
+// "reached too far" flag.  DESIGN.md "K12".
 //
 // The per-block logic is the exact step's (inflate_decode.cuh: BitReader, parse_tables, build_table, slow_decode) with
 // every end-of-input rule of the reference: a chunk reads the stream's input up to its end, not its slice's.
@@ -107,10 +109,11 @@ B200Z_HD bool ck_block_here(const uint8_t *in, uint32_t in_len, unsigned long lo
   return false;
 }
 
-// One warp per chunk: bit offsets lo[k], lo[k] + 1, ... below hi[k] are tried 32 at a time; the lowest that passes wins.
+// One warp per chunk: bit offsets lo, lo + 1, ... below hi of its stream are tried 32 at a time; the lowest that passes
+// wins.
 __global__ void __launch_bounds__(32)
-k_inflate_find_blocks(const uint8_t *__restrict__ in, uint32_t in_len, const unsigned long long *__restrict__ lo,
-                      const unsigned long long *__restrict__ hi, unsigned long long *__restrict__ cand, uint32_t n) {
+k_inflate_find_blocks(const uint8_t *__restrict__ in_base, const CkStream *__restrict__ streams,
+                      const CkFind *__restrict__ finds, unsigned long long *__restrict__ cand, uint32_t n) {
   const uint32_t k = blockIdx.x;
   if (k >= n) return;
   const int lane = threadIdx.x & 31;
@@ -118,7 +121,10 @@ k_inflate_find_blocks(const uint8_t *__restrict__ in, uint32_t in_len, const uns
   uint8_t lens[320];
   SlowTab sl;
   SlowTabD sd;
-  const unsigned long long a = lo[k], b = hi[k];
+  const CkFind fd = finds[k];
+  const uint8_t *in = in_base + streams[fd.stream].in_off;
+  const uint32_t in_len = streams[fd.stream].in_len;
+  const unsigned long long a = fd.lo, b = fd.hi;
   unsigned long long found = CK_NOCAND;
   for (unsigned long long base = a; base < b; base += 32) {
     const unsigned long long o = base + (unsigned long long)lane;
@@ -133,14 +139,18 @@ k_inflate_find_blocks(const uint8_t *__restrict__ in, uint32_t in_len, const uns
 }
 
 // One lane per chunk: decode from jobs[j].start_bit, block after block, until a block ends at or past stop_bit or a final
-// block is done.  Symbols go to 64 KiB pages taken off the pool by an atomic counter; every page records whose it is.
+// block is done.  Symbols go to 64 KiB pages taken off the stream's page range by its atomic counter
+// (page_ctr[stream]); every page records whose it is.
 __global__ void __launch_bounds__(32)
-k_inflate_chunks(const uint8_t *__restrict__ in, uint32_t in_len, const CkJob *__restrict__ jobs, uint32_t n,
-                 CkRes *__restrict__ res, uint16_t *__restrict__ pool, CkPage *__restrict__ pinfo, uint32_t *page_ctr,
-                 uint32_t n_pages) {
+k_inflate_chunks(const uint8_t *__restrict__ in_base, const CkStream *__restrict__ streams, const CkJob *__restrict__ jobs,
+                 uint32_t n, CkRes *__restrict__ res, uint16_t *__restrict__ pool, CkPage *__restrict__ pinfo,
+                 uint32_t *page_ctr) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= n) return;
   const CkJob job = jobs[j];
+  const CkStream sm = streams[job.stream];
+  const uint8_t *in = in_base + sm.in_off;
+  const uint32_t in_len = sm.in_len;
   uint16_t lut[LUT_HALFWORDS];
   uint16_t *lut_l = lut, *lut_d = lut + (1 << LBITS);
   uint8_t lens[320];
@@ -155,8 +165,9 @@ k_inflate_chunks(const uint8_t *__restrict__ in, uint32_t in_len, const CkJob *_
   // the next symbol; false when the pool is exhausted
   auto put = [&](uint32_t v) -> bool {
     if ((nsym & (CK_PAGE - 1u)) == 0u) {
-      const uint32_t p = atomicAdd(page_ctr, 1u);
-      if (p >= n_pages) return false;
+      uint32_t p = atomicAdd(page_ctr + job.stream, 1u);
+      if (p >= sm.n_pages) return false;
+      p += sm.page0;
       CkPage pi;
       pi.slot = job.slot;
       pi.seq = nsym / CK_PAGE;
@@ -313,16 +324,19 @@ __device__ __forceinline__ uint8_t ck_resolve(uint32_t v, const uint8_t *out, un
   return out[src];
 }
 
-// One CTA walks the chain in order and writes the resolved last 32 KiB of every chunk at its final place: the window of
-// chunk k + 1 is then in the output buffer when k + 1 is reached (a chunk shorter than 32 KiB reaches further back,
-// into tails written before it).
+// One CTA per stream walks its chain, chain[chain_lo[blockIdx.x] .. chain_lo[blockIdx.x + 1]), in order and writes the
+// resolved last 32 KiB of every chunk at its final place: the window of chunk k + 1 is then in the output buffer when
+// k + 1 is reached (a chunk shorter than 32 KiB reaches further back, into tails written before it).  Streams write
+// disjoint output ranges, so their CTAs do not wait on each other.
 constexpr int CK_WIN_THREADS = 256;
 constexpr int CK_WIN_PER_THREAD = (int)CK_PAGE / CK_WIN_THREADS;
 __global__ void __launch_bounds__(CK_WIN_THREADS)
-k_inflate_windows(const CkChain *__restrict__ chain, uint32_t n_chain, const uint32_t *__restrict__ flat,
-                  const uint16_t *__restrict__ pool, uint8_t *out, unsigned long long lo_valid, uint32_t *bad) {
-  for (uint32_t k = 0; k < n_chain; ++k) {
+k_inflate_windows(const CkChain *__restrict__ chain, const uint32_t *__restrict__ chain_lo, const uint32_t *__restrict__ flat,
+                  const uint16_t *__restrict__ pool, uint8_t *out, const CkStream *__restrict__ streams, uint32_t *bad) {
+  const uint32_t k0 = chain_lo[blockIdx.x], k1 = chain_lo[blockIdx.x + 1];
+  for (uint32_t k = k0; k < k1; ++k) {
     const CkChain c = chain[k];
+    const unsigned long long lo_valid = streams[c.stream].lo_valid;
     const uint32_t t = c.nsym < CK_PAGE ? c.nsym : CK_PAGE, base = c.nsym - t;
     uint32_t v[CK_WIN_PER_THREAD];
 #pragma unroll
@@ -334,19 +348,21 @@ k_inflate_windows(const CkChain *__restrict__ chain, uint32_t n_chain, const uin
 #pragma unroll
     for (int i = 0; i < CK_WIN_PER_THREAD; ++i) {
       const uint32_t x = (uint32_t)i * CK_WIN_THREADS + threadIdx.x;
-      if (x < t) out[c.out_off + base + x] = ck_resolve(v[i], out, c.out_off, lo_valid, bad);
+      if (x < t) out[c.out_off + base + x] = ck_resolve(v[i], out, c.out_off, lo_valid, bad + c.stream);
     }
     __syncthreads();
   }
 }
 
-// One CTA per page of the chain's flat page list: symbols -> bytes at their final place.  A chunk's last 32 KiB are
-// k_inflate_windows' and are left alone here: other CTAs read them as windows.
+// One CTA per page of the flat page list (every stream's chain): symbols -> bytes at their final place.  A chunk's last
+// 32 KiB are k_inflate_windows' and are left alone here: other CTAs read them as windows.  A reach before the stream's
+// allowed history raises that stream's flag only.
 __global__ void __launch_bounds__(256)
 k_inflate_emit(const CkChain *__restrict__ chain, const uint32_t *__restrict__ flat, const uint32_t *__restrict__ flat_chunk,
-               const uint16_t *__restrict__ pool, uint8_t *out, unsigned long long lo_valid, uint32_t *bad) {
+               const uint16_t *__restrict__ pool, uint8_t *out, const CkStream *__restrict__ streams, uint32_t *bad) {
   const uint32_t f = blockIdx.x;
   const CkChain c = chain[flat_chunk[f]];
+  const unsigned long long lo_valid = streams[c.stream].lo_valid;
   const uint32_t seq = f - c.page0;
   const uint32_t first = seq * CK_PAGE;
   const uint32_t body = c.nsym > CK_PAGE ? c.nsym - CK_PAGE : 0u;  // symbols in front of the tail
@@ -354,7 +370,7 @@ k_inflate_emit(const CkChain *__restrict__ chain, const uint32_t *__restrict__ f
   const uint32_t cnt = body - first < CK_PAGE ? body - first : CK_PAGE;
   const uint16_t *src = pool + (size_t)flat[f] * CK_PAGE;
   uint8_t *dst = out + c.out_off + first;
-  for (uint32_t i = threadIdx.x; i < cnt; i += blockDim.x) dst[i] = ck_resolve(src[i], out, c.out_off, lo_valid, bad);
+  for (uint32_t i = threadIdx.x; i < cnt; i += blockDim.x) dst[i] = ck_resolve(src[i], out, c.out_off, lo_valid, bad + c.stream);
 }
 
 }  // namespace b200z

@@ -394,30 +394,30 @@ cudaError_t launch_find_markers(const uint8_t *d_in, size_t n, unsigned long lon
   return cudaGetLastError();
 }
 
-// ---- K12 (inflate_chunked.cuh): one stream by many chunks ----
-cudaError_t ck_launch_find(const uint8_t *in, uint32_t in_len, const unsigned long long *lo, const unsigned long long *hi,
-                           unsigned long long *cand, uint32_t n, cudaStream_t s) {
+// ---- K12 (inflate_chunked.cuh): a batch of streams, each by many chunks ----
+cudaError_t ck_launch_find(const uint8_t *in_base, const CkStream *streams, const CkFind *finds, unsigned long long *cand,
+                           uint32_t n, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  k_inflate_find_blocks<<<n, 32, 0, s>>>(in, in_len, lo, hi, cand, n);
+  k_inflate_find_blocks<<<n, 32, 0, s>>>(in_base, streams, finds, cand, n);
   count_launch();
   return cudaGetLastError();
 }
-cudaError_t ck_launch_chunks(const uint8_t *in, uint32_t in_len, const CkJob *jobs, uint32_t n, CkRes *res, uint16_t *pool,
-                             CkPage *pinfo, uint32_t *page_ctr, uint32_t n_pages, cudaStream_t s) {
+cudaError_t ck_launch_chunks(const uint8_t *in_base, const CkStream *streams, const CkJob *jobs, uint32_t n, CkRes *res,
+                             uint16_t *pool, CkPage *pinfo, uint32_t *page_ctr, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
-  k_inflate_chunks<<<(n + 31) / 32, 32, 0, s>>>(in, in_len, jobs, n, res, pool, pinfo, page_ctr, n_pages);
+  k_inflate_chunks<<<(n + 31) / 32, 32, 0, s>>>(in_base, streams, jobs, n, res, pool, pinfo, page_ctr);
   count_launch();
   return cudaGetLastError();
 }
-cudaError_t ck_launch_resolve(const CkChain *chain, uint32_t n_chain, const uint32_t *flat, const uint32_t *flat_chunk,
-                              uint32_t n_flat, const uint16_t *pool, uint8_t *out, unsigned long long lo_valid, uint32_t *bad,
-                              cudaStream_t s) {
-  if (n_chain == 0) return cudaSuccess;
-  k_inflate_windows<<<1, CK_WIN_THREADS, 0, s>>>(chain, n_chain, flat, pool, out, lo_valid, bad);
+cudaError_t ck_launch_resolve(const CkChain *chain, const uint32_t *chain_lo, uint32_t n_walks, const uint32_t *flat,
+                              const uint32_t *flat_chunk, uint32_t n_flat, const uint16_t *pool, uint8_t *out,
+                              const CkStream *streams, uint32_t *bad, cudaStream_t s) {
+  if (n_walks == 0) return cudaSuccess;
+  k_inflate_windows<<<n_walks, CK_WIN_THREADS, 0, s>>>(chain, chain_lo, flat, pool, out, streams, bad);
   count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || n_flat == 0) return e;
-  k_inflate_emit<<<n_flat, 256, 0, s>>>(chain, flat, flat_chunk, pool, out, lo_valid, bad);
+  k_inflate_emit<<<n_flat, 256, 0, s>>>(chain, flat, flat_chunk, pool, out, streams, bad);
   count_launch();
   return cudaGetLastError();
 }

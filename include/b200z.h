@@ -191,7 +191,10 @@ int b200z_zip_comment(const uint8_t *zip, size_t zip_len, uint64_t *off, uint32_
 #define B200Z_ZIP_ENCRYPTED (-20)  /* status: encrypted member, not decoded                                      */
 #define B200Z_ZIP_TOO_LARGE (-21)  /* status: member of 4 GiB or more                                            */
 /* Member i is written to out[out_off[i] .. +out_room[i]); out_len[i] = bytes it produced (may exceed the room:
- * status B200Z_U_NOSPC), status[i] = B200Z_U_* / B200Z_ZIP_*.                                                    */
+ * status B200Z_U_NOSPC), status[i] = B200Z_U_* / B200Z_ZIP_*.  All members are decoded in one call: deflate members
+ * as units of one inflate batch, except that a member of 16 MiB compressed or more without full-flush points is decoded
+ * across the whole GPU by many chunks at once (several such members together).  Which path decodes a member never
+ * changes its bytes, out_len or status.                                                                           */
 int b200z_zip_extract(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                       size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
                       int32_t *status, uint32_t flags);

@@ -76,6 +76,8 @@ _SIGS = {
     "b200z_gzip_encode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_uint32, C.c_void_p, C.c_size_t,
                                     C.POINTER(C.c_size_t)]),
     "b200z_bzip2_decode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "b200z_bzip2_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_crc32": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]),
     "b200z_xz_decode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_xz_bound": (C.c_size_t, [C.c_void_p, C.c_size_t]),

@@ -201,6 +201,58 @@ class BZip2Decoder:
         return _stream_result(rc)
 
 
+def bzip2_decode_batch(streams, verify: bool = False) -> list:
+    """BZip2Decoder().decodeBytes(stream, verify:) for every stream of `streams` in one b200z_bzip2_decode_batch call:
+    a list of (rc, bytes) in the same order.  rc is what b200z_bzip2_decode gives for that stream alone: OK, E_DATA
+    (decodeStream returned false; bytes = the blocks decoded before the failure) or E_THROW (the reference throws a
+    RangeError).  Each output room starts at BZip2Decoder's first guess; only the streams that did not fit are decoded
+    again, in larger rooms."""
+    L = _ffi.ensure_init()
+    views = [memoryview(s).cast("B") for s in streams]
+    n = len(views)
+    if n == 0:
+        return []
+    in_off = (C.c_uint64 * n)()
+    in_len = (C.c_uint64 * n)()
+    pos = 0
+    for i, v in enumerate(views):
+        in_off[i], in_len[i] = pos, len(v)
+        pos += len(v)
+    in_buf = (C.c_uint8 * max(pos, 1))()
+    for i, v in enumerate(views):
+        C.memmove(C.addressof(in_buf) + in_off[i], bytes(v), len(v))
+    rooms = [max(6 * len(v) + 4096, 1 << 12) for v in views]
+    result = [None] * n
+    todo = list(range(n))
+    while todo:
+        m = len(todo)
+        a_in_off = (C.c_uint64 * m)(*[in_off[i] for i in todo])
+        a_in_len = (C.c_uint64 * m)(*[in_len[i] for i in todo])
+        a_out_off = (C.c_uint64 * m)()
+        a_cap = (C.c_uint64 * m)(*[rooms[i] for i in todo])
+        total = 0
+        for k in range(m):
+            a_out_off[k] = total
+            total += a_cap[k]
+        out = (C.c_uint8 * max(total, 1))()
+        a_len = (C.c_uint64 * m)()
+        a_rc = (C.c_int32 * m)()
+        _ffi.check(L.b200z_bzip2_decode_batch(C.addressof(in_buf), a_in_off, a_in_len, m, int(verify), C.addressof(out), a_out_off,
+                                              a_cap, a_len, a_rc))
+        again = []
+        for k, i in enumerate(todo):
+            rc, got = a_rc[k], a_len[k]
+            if rc == _ffi.E_NOSPC and rooms[i] < (1 << 40):
+                rooms[i] = max(rooms[i] * 2, got + (got >> 3))
+                again.append(i)
+                continue
+            if rc not in (_ffi.OK, _ffi.E_DATA, _ffi.E_THROW):
+                _ffi.check(rc)
+            result[i] = (rc, C.string_at(C.addressof(out) + a_out_off[k], got))
+        todo = again
+    return result
+
+
 class BZip2Encoder:
     """BZip2Encoder().encodeBytes / encode / encodeStream (lib/src/codecs/bzip2_encoder.dart:15-81): one "BZh9"
     stream; encodeStream returns True."""

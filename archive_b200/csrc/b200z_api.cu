@@ -1397,13 +1397,6 @@ struct Carver {  // carve typed arrays out of one device allocation
   }
 };
 
-static inline uint32_t be32_at_bit(const uint8_t *in, size_t n, uint64_t bit) {
-  uint64_t v = 0;
-  size_t b0 = (size_t)(bit >> 3);
-  for (int i = 0; i < 5; ++i) v = (v << 8) | (b0 + i < n ? in[b0 + i] : 0);
-  return (uint32_t)(v >> (8 - (bit & 7)));
-}
-
 // shard != nullptr: decode only this rank's share of the block candidates and report every block instead of walking the
 // chain (the ranks' reports are merged and validated by the caller, archive_b200/shard.py).
 struct Bz2Shard {
@@ -1411,430 +1404,593 @@ struct Bz2Shard {
   b200z_bz2_block *blocks;
   size_t blocks_cap, n_blocks;
 };
-static int bzip2_decode_impl(const uint8_t *in, size_t in_len, int verify, uint8_t *out, size_t out_cap, size_t *out_len,
-                             Bz2Shard *shard = nullptr) {
-  *out_len = 0;
-  // 'B' 'Z' 'h' level: each is a readByte() that throws at EOS (bz2_bit_reader.dart:17-20)
-  static const uint8_t sig[3] = {0x42, 0x5a, 0x68};
-  for (int i = 0; i < 3; ++i) {
-    if ((size_t)i >= in_len) {
-      set_err("bzip2: truncated signature (Dart: RangeError)");
-      return B200Z_E_THROW;
-    }
-    if (in[i] != sig[i]) {
-      set_err("bzip2: bad signature");
-      return B200Z_E_DATA;
-    }
-  }
-  if (in_len < 4) {
-    set_err("bzip2: truncated header (Dart: RangeError)");
-    return B200Z_E_THROW;
-  }
-  const int level = (int)in[3] - 0x30;
-  if (level < 0 || level > 9) {
-    set_err("bzip2: bad block size");
-    return B200Z_E_DATA;
-  }
-  if (in_len == 4) return B200Z_OK;  // while (!input.isEOS) never runs
-  const uint32_t nblock_max = (uint32_t)level * 100000u;
-  const uint64_t total_bits = (uint64_t)in_len * 8;
 
-  int rc = stage_input(in, in_len);
-  if (rc) return rc;
-  CU(cudaMemsetAsync((uint8_t *)g.d_in.p + in_len, 0, 64, g.stream));
+// One stream of a batch: its bytes d_base[in_off, +in_len) on the device, its output slot on the host, and what
+// decodeStream makes of it (rc, out_len: what b200z_bzip2_decode returns and reports for the stream alone).
+struct Bz2Job {
+  uint64_t in_off, in_len;
+  uint8_t *out;
+  size_t out_cap;
+  size_t out_len;
+  int rc;
+};
 
-  // ---- K6: candidates ----
-  const uint32_t cand_cap = 1u << 20;
-  CU(g.d_small.reserve((size_t)cand_cap * 8 + 256));
-  unsigned long long *d_cand = (unsigned long long *)((uint8_t *)g.d_small.p + 256);
-  uint32_t *d_ncand = (uint32_t *)g.d_small.p;
-  CU(bz2_launch_scan((const uint8_t *)g.d_in.p, in_len, d_cand, d_ncand, cand_cap, g.stream));
-  uint32_t ncand = 0;
-  CU(cudaMemcpyAsync(&ncand, d_ncand, 4, cudaMemcpyDeviceToHost, g.stream));
-  CU(cudaStreamSynchronize(g.stream));
-  if (ncand > cand_cap) {
-    set_err("bzip2: more than %u magic candidates", cand_cap);
-    return B200Z_E_INTERNAL;
+// (test hooks) cap on the blocks of one device group (0: the memory budget alone); the last call's streams, device groups
+// and blocks
+static uint32_t g_bz2_max_group_blocks = 0;
+static unsigned long long g_bz2_stats[3];
+// Device memory a group of streams may take for K7/K8 workspace and output slots, unless the buffers already hold more.
+// One stream that needs more runs as a group of its own.
+constexpr size_t BZ2_GROUP_BUDGET = (size_t)8 << 30;
+
+struct Bz2Arrays {
+  unsigned long long *blk_bit, *blk_end, *end_bit, *block_out, *block_off;
+  uint32_t *blk_lim, *rec_val, *rec_pos, *n_rec, *nblock, *orig_ptr, *rnd, *chist, *tt, *seg_len, *seg_next, *seg_off, *seg_resume,
+      *slice_state, *slice_out, *block_crc, *cycle_len, *fast, *walk_ctr;
+  int32_t *status, *irregular;
+  uint8_t *sym8, *raw, *slots;
+  BzChainHost *chain;
+  size_t bytes;
+};
+// nb_all candidate blocks, the big per-block arrays for nbk of them at a stride of `stride` (the largest level x 100000 of
+// the group's streams)
+static Bz2Arrays bz2_carve(void *base, uint32_t nb_all, uint32_t nbk, uint32_t stride) {
+  Carver c(base);
+  const uint32_t chunks_max = (stride + 1023) / 1024;
+  Bz2Arrays a;
+  a.blk_bit = c.take<unsigned long long>(nb_all);
+  a.blk_end = c.take<unsigned long long>(nb_all);
+  a.blk_lim = c.take<uint32_t>(nb_all);
+  a.end_bit = c.take<unsigned long long>(nbk);
+  a.block_out = c.take<unsigned long long>(nbk);
+  a.block_off = c.take<unsigned long long>(nbk + 1);
+  a.n_rec = c.take<uint32_t>(nbk);
+  a.nblock = c.take<uint32_t>(nbk);
+  a.orig_ptr = c.take<uint32_t>(nbk);
+  a.rnd = c.take<uint32_t>(nbk);
+  a.status = c.take<int32_t>(nbk);
+  a.irregular = c.take<int32_t>(nbk);
+  a.block_crc = c.take<uint32_t>(nbk);
+  a.cycle_len = c.take<uint32_t>(nbk);
+  a.fast = c.take<uint32_t>(nbk);
+  a.walk_ctr = c.take<uint32_t>(4);
+  a.chain = c.take<BzChainHost>(nbk);
+  a.seg_len = c.take<uint32_t>((size_t)nbk * 4098);
+  a.seg_next = c.take<uint32_t>((size_t)nbk * 4098);
+  a.seg_off = c.take<uint32_t>((size_t)nbk * 4098);
+  a.seg_resume = c.take<uint32_t>((size_t)nbk * 4098);
+  a.slice_state = c.take<uint32_t>((size_t)nbk * 1024);
+  a.slice_out = c.take<uint32_t>((size_t)nbk * 1024);
+  a.chist = c.take<uint32_t>((size_t)nbk * chunks_max * 256);
+  a.rec_val = c.take<uint32_t>((size_t)nbk * stride);
+  a.rec_pos = c.take<uint32_t>((size_t)nbk * stride);
+  a.tt = c.take<uint32_t>((size_t)nbk * stride);
+  a.sym8 = c.take<uint8_t>((size_t)nbk * stride);
+  a.raw = c.take<uint8_t>((size_t)nbk * stride);
+  a.slots = c.take<uint8_t>((size_t)nbk * bz2_slot_bytes_per_block());
+  a.bytes = align_up(c.off, 256);
+  return a;
+}
+
+// the 32 bits from `bit` on (big-endian; bytes past the end read 0) of a stream of `len` bytes, for a bit among its last 48:
+// they lie in its last 8 bytes, which are all the host has of it
+static inline uint32_t be32_in_tail(const uint8_t *tail8, uint64_t len, uint64_t bit) {
+  uint64_t v = 0;
+  const uint64_t b0 = bit >> 3;
+  for (int i = 0; i < 5; ++i) {
+    const uint64_t j = b0 + i;
+    v = (v << 8) | (j < len && j + 8 >= len ? tail8[j + 8 - len] : 0u);
   }
-  std::vector<unsigned long long> cand(ncand);
-  if (ncand) CU(cudaMemcpy(cand.data(), d_cand, (size_t)ncand * 8, cudaMemcpyDeviceToHost));
-  std::sort(cand.begin(), cand.end(), [](unsigned long long a, unsigned long long b) {
-    return (a & ~(1ull << 63)) < (b & ~(1ull << 63));
-  });
-  std::vector<unsigned long long> blk_bits;
-  std::vector<uint32_t> blk_of_cand(ncand, 0xffffffffu);
-  for (uint32_t i = 0; i < ncand; ++i)
-    if (!(cand[i] >> 63)) {
-      blk_of_cand[i] = (uint32_t)blk_bits.size();
-      blk_bits.push_back(cand[i]);
-    }
-  const uint32_t nb = (uint32_t)blk_bits.size();
+  return (uint32_t)(v >> (8 - (bit & 7)));
+}
 
-  // ---- device arrays ----
-  const uint32_t chunks_max = (nblock_max + 1023) / 1024;
-  const uint32_t nb_all = nb ? nb : 1;
-  auto carve = [&](void *base, uint32_t nbk) {
+// BZip2Decoder.decodeStream for n streams whose bytes are on the device already.  K6 scans all of them in one launch; the
+// streams are then cut into consecutive device groups that fit the memory budget, and each group takes one K7 and one K8
+// over the blocks of all its streams, each stream's output going to a slot of its own.  Returns B200Z_OK unless the device
+// fails; each stream's result is in its job.
+static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, int verify, Bz2Shard *shard = nullptr) {
+  g_bz2_stats[0] = n;
+  g_bz2_stats[1] = g_bz2_stats[2] = 0;
+  if (n == 0) return B200Z_OK;
+
+  // ---- K6: candidates of every stream, with their stream, their stored CRC and the streams' first and last bytes ----
+  std::vector<Bz2ScanStream> h_str(n);
+  std::vector<unsigned long long> h_thr(n + 1, 0);
+  for (size_t i = 0; i < n; ++i) {
+    jobs[i].out_len = 0;
+    jobs[i].rc = B200Z_OK;
+    h_str[i] = {jobs[i].in_off, jobs[i].in_len};
+    h_thr[i + 1] = h_thr[i] + std::max<uint64_t>(1, (jobs[i].in_len + 3) / 4);
+  }
+  auto scan_layout = [&](void *base, uint32_t cap, size_t *bytes) {
     Carver c(base);
-    struct A {
-      unsigned long long *blk_bit, *end_bit, *block_out, *block_off;
-      uint32_t *rec_val, *rec_pos, *n_rec, *nblock, *orig_ptr, *rnd, *chist, *tt, *seg_len, *seg_next, *seg_off, *seg_resume, *slice_state,
-          *slice_out, *block_crc, *cycle_len, *fast, *walk_ctr;
-      int32_t *status, *irregular;
-      uint8_t *sym8, *raw, *slots;
-      BzChainHost *chain;
-      size_t bytes;
-    } a;
-    a.blk_bit = c.take<unsigned long long>(nb_all);
-    a.end_bit = c.take<unsigned long long>(nbk);
-    a.block_out = c.take<unsigned long long>(nbk);
-    a.block_off = c.take<unsigned long long>(nbk + 1);
-    a.n_rec = c.take<uint32_t>(nbk);
-    a.nblock = c.take<uint32_t>(nbk);
-    a.orig_ptr = c.take<uint32_t>(nbk);
-    a.rnd = c.take<uint32_t>(nbk);
-    a.status = c.take<int32_t>(nbk);
-    a.irregular = c.take<int32_t>(nbk);
-    a.block_crc = c.take<uint32_t>(nbk);
-    a.cycle_len = c.take<uint32_t>(nbk);
-    a.fast = c.take<uint32_t>(nbk);
-    a.walk_ctr = c.take<uint32_t>(4);
-    a.chain = c.take<BzChainHost>(nbk);
-    a.seg_len = c.take<uint32_t>((size_t)nbk * 4098);
-    a.seg_next = c.take<uint32_t>((size_t)nbk * 4098);
-    a.seg_off = c.take<uint32_t>((size_t)nbk * 4098);
-    a.seg_resume = c.take<uint32_t>((size_t)nbk * 4098);
-    a.slice_state = c.take<uint32_t>((size_t)nbk * 1024);
-    a.slice_out = c.take<uint32_t>((size_t)nbk * 1024);
-    a.chist = c.take<uint32_t>((size_t)nbk * chunks_max * 256);
-    a.rec_val = c.take<uint32_t>((size_t)nbk * nblock_max);
-    a.rec_pos = c.take<uint32_t>((size_t)nbk * nblock_max);
-    a.tt = c.take<uint32_t>((size_t)nbk * nblock_max);
-    a.sym8 = c.take<uint8_t>((size_t)nbk * nblock_max);
-    a.raw = c.take<uint8_t>((size_t)nbk * nblock_max);
-    a.slots = c.take<uint8_t>((size_t)nbk * bz2_slot_bytes_per_block());
-    a.bytes = align_up(c.off, 256);
+    Bz2Scan a;
+    a.in = d_base;
+    a.n_streams = (uint32_t)n;
+    a.cap = cap;
+    a.n_cand = c.take<uint32_t>(1);
+    a.streams = c.take<Bz2ScanStream>(n);
+    a.first_thr = c.take<unsigned long long>(n + 1);
+    a.ends = c.take<uint8_t>(n * 12);
+    a.cand = c.take<unsigned long long>(cap);
+    a.cand_stream = c.take<uint32_t>(cap);
+    a.cand_crc = c.take<uint32_t>(cap);
+    *bytes = align_up(c.off, 256);
     return a;
   };
-  uint32_t nbk = nb ? nb : 1;
-  if (shard) {  // only this rank's share needs the big per-block arrays (blk_bit keeps all candidates: small)
-    const uint32_t lo = (uint32_t)((uint64_t)nb * shard->rank / shard->world), hi = (uint32_t)((uint64_t)nb * (shard->rank + 1) / shard->world);
-    nbk = hi > lo ? hi - lo : 1;
+  const uint32_t cand_cap = 1u << 20;  // per stream
+  uint32_t cap = cand_cap, ncand = 0;
+  Bz2Scan sc;
+  for (;;) {
+    size_t bytes = 0;
+    scan_layout(nullptr, cap, &bytes);
+    CU(g.d_small.reserve(bytes));
+    sc = scan_layout(g.d_small.p, cap, &bytes);
+    CU(cudaMemcpyAsync((void *)sc.streams, h_str.data(), n * sizeof(Bz2ScanStream), cudaMemcpyHostToDevice, g.stream));
+    CU(cudaMemcpyAsync((void *)sc.first_thr, h_thr.data(), (n + 1) * 8, cudaMemcpyHostToDevice, g.stream));
+    CU(bz2_launch_scan_streams(sc, h_thr[n], g.stream));
+    CU(cudaMemcpyAsync(&ncand, sc.n_cand, 4, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+    if (ncand <= cap) break;
+    cap = ncand;  // (more candidates than the buffer holds: once more with room for all of them)
   }
-  auto sz = carve(nullptr, nbk);
-  CU(g.d_bz.reserve(sz.bytes));
-  auto A = carve(g.d_bz.p, nbk);
+  std::vector<unsigned long long> h_cand(ncand);
+  std::vector<uint32_t> h_cstr(ncand), h_ccrc(ncand);
+  std::vector<uint8_t> ends(n * 12);
+  if (ncand) {
+    CU(cudaMemcpyAsync(h_cand.data(), sc.cand, (size_t)ncand * 8, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaMemcpyAsync(h_cstr.data(), sc.cand_stream, (size_t)ncand * 4, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaMemcpyAsync(h_ccrc.data(), sc.cand_crc, (size_t)ncand * 4, cudaMemcpyDeviceToHost, g.stream));
+  }
+  CU(cudaMemcpyAsync(ends.data(), sc.ends, n * 12, cudaMemcpyDeviceToHost, g.stream));
+  CU(cudaStreamSynchronize(g.stream));
+  // candidates by stream, then by bit; positions from here on are bits of their stream (| end-of-stream << 63)
+  std::vector<uint32_t> order(ncand);
+  for (uint32_t i = 0; i < ncand; ++i) order[i] = i;
+  const unsigned long long POS = ~(1ull << 63);
+  std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+    return h_cstr[a] != h_cstr[b] ? h_cstr[a] < h_cstr[b] : (h_cand[a] & POS) < (h_cand[b] & POS);
+  });
+  std::vector<unsigned long long> cand(ncand);
+  std::vector<uint32_t> ccrc(ncand);
+  std::vector<uint32_t> c_lo(n + 1, 0);
+  for (uint32_t i = 0; i < ncand; ++i) {
+    const uint32_t o = order[i], s = h_cstr[o];
+    cand[i] = h_cand[o] - jobs[s].in_off * 8;
+    ccrc[i] = h_ccrc[o];
+    c_lo[s + 1]++;
+  }
+  for (size_t s = 0; s < n; ++s) c_lo[s + 1] += c_lo[s];
 
-  // ---- K7 on every candidate (speculative: a magic-looking bit pattern inside a block just decodes to junk) ----
-  std::vector<uint32_t> h_nrec(nb), h_nblock(nb), h_optr(nb), h_rnd(nb);
-  std::vector<unsigned long long> h_end(nb);
-  std::vector<int32_t> h_st(nb);
-  uint32_t k_lo = 0, k_hi = nb;  // candidates this call decodes
-  if (shard) {
-    k_lo = (uint32_t)((uint64_t)nb * shard->rank / shard->world);
-    k_hi = (uint32_t)((uint64_t)nb * (shard->rank + 1) / shard->world);
-  }
-  if (k_hi > k_lo) {
-    CU(cudaMemcpyAsync(A.blk_bit, blk_bits.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, g.stream));
-    Bz2Entropy e;
-    e.words = (const uint32_t *)g.d_in.p;
-    e.n_bytes = in_len;
-    e.blk_bit = A.blk_bit + k_lo;
-    e.n_blocks = k_hi - k_lo;
-    e.nblock_max = nblock_max;
-    // block k of this call uses slot k - k_lo of every per-block array
-    e.rec_val = A.rec_val; e.rec_pos = A.rec_pos; e.n_rec = A.n_rec; e.nblock = A.nblock; e.orig_ptr = A.orig_ptr;
-    e.randomised = A.rnd; e.end_bit = A.end_bit; e.status = A.status; e.fast_flag = A.fast; e.sym8 = A.sym8;
-    CU(bz2_launch_entropy(e, g.stream));
-    const uint32_t m = k_hi - k_lo;
-    auto fetch = [&]() -> int {
-      CU(cudaMemcpyAsync(h_nrec.data() + k_lo, A.n_rec, m * 4, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaMemcpyAsync(h_nblock.data() + k_lo, A.nblock, m * 4, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaMemcpyAsync(h_optr.data() + k_lo, A.orig_ptr, m * 4, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaMemcpyAsync(h_rnd.data() + k_lo, A.rnd, m * 4, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaMemcpyAsync(h_end.data() + k_lo, A.end_bit, (size_t)m * 8, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaMemcpyAsync(h_st.data() + k_lo, A.status, m * 4, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaStreamSynchronize(g.stream));
-      return B200Z_OK;
-    };
-    rc = fetch();
-    if (rc) return rc;
-    {
-      std::vector<uint32_t> h_fast(m);
-      CU(cudaMemcpy(h_fast.data(), A.fast, (size_t)m * 4, cudaMemcpyDeviceToHost));
-      unsigned long long nf = 0;
-      for (uint32_t v : h_fast) nf += v;
-      g_bz2_fast_blocks += nf;
-      g_bz2_exact_blocks += m - nf;
-    }
-    // damaged blocks that the reference keeps decoding past a bad Huffman code (K7 status -3): decoded again the reference's
-    // way, one thread each (bzip2_kernels.cu: k_bz2_entropy_literal); intact streams have none
-    std::vector<uint32_t> quirk;
-    for (uint32_t k = k_lo; k < k_hi; ++k)
-      if (h_st[k] == -3) quirk.push_back(k - k_lo);
-    if (!quirk.empty()) {
-      uint32_t *d_list = (uint32_t *)((uint8_t *)g.d_small.p + 256);  // the candidate list is on the host by now
-      CU(cudaMemcpyAsync(d_list, quirk.data(), quirk.size() * 4, cudaMemcpyHostToDevice, g.stream));
-      CU(bz2_launch_entropy_literal(e, d_list, (uint32_t)quirk.size(), g.stream));
-      rc = fetch();
-      if (rc) return rc;
-    }
-  }
-
-  // ---- walk the chain exactly as decodeStream's loop does (:46-87) ----
-  std::vector<BzChainHost> chain;
-  std::vector<uint32_t> stored_crc;
-  int final_rc = B200Z_OK;
-  bool have_eos = false;
-  uint32_t eos_crc = 0;
-  uint64_t pos = 32;
-  size_t ci = 0;
-  std::vector<uint32_t> chain_of(nb, 0xffffffffu);
-  if (shard) {
-    for (uint32_t k = k_lo; k < k_hi; ++k)
-      if (h_st[k] == 0) {
-        chain_of[k] = (uint32_t)chain.size();
-        chain.push_back({k - k_lo, h_nblock[k], h_nrec[k], h_optr[k], h_rnd[k] ? 1u : 0u});
-        stored_crc.push_back(blk_bits[k] + 80 <= total_bits ? be32_at_bit(in, in_len, blk_bits[k] + 48) : 0u);
+  // ---- stream headers: 'B' 'Z' 'h' level, each a readByte() that throws at EOS (bz2_bit_reader.dart:17-20) ----
+  std::vector<uint32_t> lim(n, 0), nblk(n, 0);
+  std::vector<char> live(n, 0);
+  static const uint8_t sig[3] = {0x42, 0x5a, 0x68};
+  for (size_t s = 0; s < n; ++s) {
+    const uint8_t *hd = ends.data() + s * 12;
+    const uint64_t len = jobs[s].in_len;
+    int r = B200Z_OK;
+    for (int i = 0; i < 3 && r == B200Z_OK; ++i) {
+      if ((uint64_t)i >= len) {
+        set_err("bzip2: truncated signature (Dart: RangeError)");
+        r = B200Z_E_THROW;
+      } else if (hd[i] != sig[i]) {
+        set_err("bzip2: bad signature");
+        r = B200Z_E_DATA;
       }
+    }
+    if (r == B200Z_OK && len < 4) {
+      set_err("bzip2: truncated header (Dart: RangeError)");
+      r = B200Z_E_THROW;
+    }
+    const int level = (int)hd[3] - 0x30;
+    if (r == B200Z_OK && (level < 0 || level > 9)) {
+      set_err("bzip2: bad block size");
+      r = B200Z_E_DATA;
+    }
+    if (r == B200Z_OK && c_lo[s + 1] - c_lo[s] > cand_cap) {
+      set_err("bzip2: more than %u magic candidates", cand_cap);
+      r = B200Z_E_INTERNAL;
+    }
+    jobs[s].rc = r;
+    if (r != B200Z_OK || len == 4) continue;  // (len 4: while (!input.isEOS) never runs)
+    live[s] = 1;
+    lim[s] = (uint32_t)level * 100000u;
+    for (uint32_t c = c_lo[s]; c < c_lo[s + 1]; ++c) nblk[s] += (cand[c] >> 63) ? 0u : 1u;
   }
-  for (; !shard;) {
-    if ((pos + 7) / 8 >= in_len) break;  // input.isEOS: every byte has been pulled into the bit reader
-    if (pos + 48 > total_bits) {
-      // _readBlockType (:90-111) reads its 6 bytes one at a time: the first one that fits neither magic returns -1 before
-      // the missing bytes are asked for (RangeError)
-      static const uint8_t blk_magic[6] = {0x31, 0x41, 0x59, 0x26, 0x53, 0x59}, eos_magic[6] = {0x17, 0x72, 0x45, 0x38, 0x50, 0x90};
-      bool blk = true, eos = true, mismatch = false;
-      for (int i = 0; i < 6 && pos + 8 * (uint64_t)(i + 1) <= total_bits; ++i) {
-        const uint8_t b = (uint8_t)(be32_at_bit(in, in_len, pos + 8 * (uint64_t)i) >> 24);
-        blk = blk && b == blk_magic[i];
-        eos = eos && b == eos_magic[i];
-        if (!blk && !eos) {
-          mismatch = true;
+
+  size_t budget = g.d_bz.cap + g.d_out.cap, free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess) budget = std::max(budget, std::min(free_b / 2, BZ2_GROUP_BUDGET));
+  std::vector<size_t> grp;
+  for (size_t s0 = 0; s0 < n;) {
+    // ---- the next device group: consecutive streams whose workspace and output slots fit the budget ----
+    grp.clear();
+    uint32_t nb = 0, stride = 0;
+    size_t room = 0;
+    for (; s0 < n; ++s0) {
+      if (!live[s0]) continue;
+      const uint32_t nb2 = nb + nblk[s0], stride2 = std::max(stride, lim[s0]);
+      const size_t room2 = room + jobs[s0].out_cap;
+      if (!grp.empty() && ((g_bz2_max_group_blocks && nb2 > g_bz2_max_group_blocks) ||
+                           bz2_carve(nullptr, std::max(nb2, 1u), std::max(nb2, 1u), stride2).bytes + room2 > budget))
+        break;
+      grp.push_back(s0);
+      nb = nb2;
+      stride = stride2;
+      room = room2;
+    }
+    if (grp.empty()) break;
+    const size_t G = grp.size();
+    g_bz2_stats[1]++;
+    g_bz2_stats[2] += nb;
+
+    // blocks of the group, stream after stream; blk_of[c] = the block a candidate is (for block candidates)
+    std::vector<unsigned long long> blk_bits, blk_end;
+    std::vector<uint32_t> blk_lim, blk_crc, blk_of(ncand, 0xffffffffu);
+    for (size_t s : grp)
+      for (uint32_t c = c_lo[s]; c < c_lo[s + 1]; ++c)
+        if (!(cand[c] >> 63)) {
+          blk_of[c] = (uint32_t)blk_bits.size();
+          blk_bits.push_back(jobs[s].in_off * 8 + cand[c]);
+          blk_end.push_back((jobs[s].in_off + jobs[s].in_len) * 8);
+          blk_lim.push_back(lim[s]);
+          blk_crc.push_back(cand[c] + 80 <= jobs[s].in_len * 8 ? ccrc[c] : 0u);
+        }
+    const uint32_t nb_all = nb ? nb : 1;
+    uint32_t k_lo = 0, k_hi = nb;  // candidates this call decodes
+    if (shard) {
+      k_lo = (uint32_t)((uint64_t)nb * shard->rank / shard->world);
+      k_hi = (uint32_t)((uint64_t)nb * (shard->rank + 1) / shard->world);
+    }
+    const uint32_t nbk = k_hi > k_lo ? k_hi - k_lo : 1;  // (a shard needs the big per-block arrays for its share only)
+    CU(g.d_bz.reserve(bz2_carve(nullptr, nb_all, nbk, stride).bytes));
+    const Bz2Arrays A = bz2_carve(g.d_bz.p, nb_all, nbk, stride);
+
+    // ---- K7 on every candidate (speculative: a magic-looking bit pattern inside a block just decodes to junk) ----
+    std::vector<uint32_t> h_nrec(nb), h_nblock(nb), h_optr(nb), h_rnd(nb);
+    std::vector<unsigned long long> h_end(nb);
+    std::vector<int32_t> h_st(nb);
+    if (k_hi > k_lo) {
+      CU(cudaMemcpyAsync(A.blk_bit, blk_bits.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemcpyAsync(A.blk_end, blk_end.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, g.stream));
+      CU(cudaMemcpyAsync(A.blk_lim, blk_lim.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, g.stream));
+      Bz2Entropy e;
+      e.words = (const uint32_t *)d_base;
+      e.n_bytes = 0;  // (every block has its stream's end in blk_end)
+      e.blk_bit = A.blk_bit + k_lo;
+      e.blk_end = A.blk_end + k_lo;
+      e.blk_lim = A.blk_lim + k_lo;
+      e.n_blocks = k_hi - k_lo;
+      e.nblock_max = stride;
+      // block k of this call uses slot k - k_lo of every per-block array
+      e.rec_val = A.rec_val; e.rec_pos = A.rec_pos; e.n_rec = A.n_rec; e.nblock = A.nblock; e.orig_ptr = A.orig_ptr;
+      e.randomised = A.rnd; e.end_bit = A.end_bit; e.status = A.status; e.fast_flag = A.fast; e.sym8 = A.sym8;
+      CU(bz2_launch_entropy(e, g.stream));
+      const uint32_t m = k_hi - k_lo;
+      auto fetch = [&]() -> int {
+        CU(cudaMemcpyAsync(h_nrec.data() + k_lo, A.n_rec, m * 4, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaMemcpyAsync(h_nblock.data() + k_lo, A.nblock, m * 4, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaMemcpyAsync(h_optr.data() + k_lo, A.orig_ptr, m * 4, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaMemcpyAsync(h_rnd.data() + k_lo, A.rnd, m * 4, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaMemcpyAsync(h_end.data() + k_lo, A.end_bit, (size_t)m * 8, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaMemcpyAsync(h_st.data() + k_lo, A.status, m * 4, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaStreamSynchronize(g.stream));
+        return B200Z_OK;
+      };
+      int rc = fetch();
+      if (rc) return rc;
+      {
+        std::vector<uint32_t> h_fast(m);
+        CU(cudaMemcpy(h_fast.data(), A.fast, (size_t)m * 4, cudaMemcpyDeviceToHost));
+        unsigned long long nf = 0;
+        for (uint32_t v : h_fast) nf += v;
+        g_bz2_fast_blocks += nf;
+        g_bz2_exact_blocks += m - nf;
+      }
+      // damaged blocks that the reference keeps decoding past a bad Huffman code (K7 status -3): decoded again the reference's
+      // way, one thread each (bzip2_kernels.cu: k_bz2_entropy_literal); intact streams have none
+      std::vector<uint32_t> quirk;
+      for (uint32_t k = k_lo; k < k_hi; ++k)
+        if (h_st[k] == -3) quirk.push_back(k - k_lo);
+      if (!quirk.empty()) {
+        uint32_t *d_list = (uint32_t *)((uint8_t *)g.d_small.p + 256);  // the scan's arrays are on the host by now
+        CU(cudaMemcpyAsync(d_list, quirk.data(), quirk.size() * 4, cudaMemcpyHostToDevice, g.stream));
+        CU(bz2_launch_entropy_literal(e, d_list, (uint32_t)quirk.size(), g.stream));
+        rc = fetch();
+        if (rc) return rc;
+      }
+    }
+
+    // ---- walk each stream's chain exactly as decodeStream's loop does (:46-87) ----
+    std::vector<BzChainHost> chain;
+    std::vector<uint32_t> stored_crc, ch_lo(G + 1, 0), eos_crc(G, 0);
+    std::vector<char> have_eos(G, 0);
+    std::vector<int> s_rc(G, B200Z_OK);
+    std::vector<unsigned long long> s_lo(G), s_hi(G);  // each stream's output slot in g.d_out
+    std::vector<uint32_t> chain_of(nb, 0xffffffffu);
+    size_t dev_room = 0;
+    for (size_t q = 0; q < G; ++q) {
+      const size_t s = grp[q];
+      s_lo[q] = dev_room;
+      dev_room += jobs[s].out_cap;
+      s_hi[q] = dev_room;
+      ch_lo[q] = (uint32_t)chain.size();
+      const uint64_t in_len = jobs[s].in_len, total_bits = in_len * 8, base_bit = jobs[s].in_off * 8;
+      auto push_block = [&](uint32_t k, uint32_t crc) {
+        chain_of[k] = (uint32_t)chain.size();
+        BzChainHost ce{k - k_lo, h_nblock[k], h_nrec[k], h_optr[k], h_rnd[k] ? 1u : 0u};  // randomised: serial walk in K8
+        if (chain.size() == ch_lo[q]) ce.flags |= 2u;
+        ce.out_lo = s_lo[q];
+        ce.out_hi = s_hi[q];
+        chain.push_back(ce);
+        stored_crc.push_back(crc);
+      };
+      if (shard) {
+        for (uint32_t k = k_lo; k < k_hi; ++k)
+          if (h_st[k] == 0) push_block(k, blk_crc[k]);
+        continue;
+      }
+      const uint8_t *tail = ends.data() + s * 12 + 4;
+      int final_rc = B200Z_OK;
+      uint64_t pos = 32;
+      uint32_t ci = c_lo[s];
+      const uint32_t c_end = c_lo[s + 1];
+      for (;;) {
+        if ((pos + 7) / 8 >= in_len) break;  // input.isEOS: every byte has been pulled into the bit reader
+        if (pos + 48 > total_bits) {
+          // _readBlockType (:90-111) reads its 6 bytes one at a time: the first one that fits neither magic returns -1 before
+          // the missing bytes are asked for (RangeError)
+          static const uint8_t blk_magic[6] = {0x31, 0x41, 0x59, 0x26, 0x53, 0x59}, eos_magic[6] = {0x17, 0x72, 0x45, 0x38, 0x50, 0x90};
+          bool blk = true, eos = true, mismatch = false;
+          for (int i = 0; i < 6 && pos + 8 * (uint64_t)(i + 1) <= total_bits; ++i) {
+            const uint8_t b = (uint8_t)(be32_in_tail(tail, in_len, pos + 8 * (uint64_t)i) >> 24);
+            blk = blk && b == blk_magic[i];
+            eos = eos && b == eos_magic[i];
+            if (!blk && !eos) {
+              mismatch = true;
+              break;
+            }
+          }
+          if (mismatch) {
+            set_err("bzip2: no block signature at bit %llu", (unsigned long long)pos);
+            final_rc = B200Z_E_DATA;
+          } else {
+            set_err("bzip2: truncated block header (Dart: RangeError)");
+            final_rc = B200Z_E_THROW;
+          }
           break;
         }
+        while (ci < c_end && (cand[ci] & POS) < pos) ++ci;
+        if (ci >= c_end || (cand[ci] & POS) != pos) {
+          set_err("bzip2: no block signature at bit %llu", (unsigned long long)pos);
+          final_rc = B200Z_E_DATA;  // _readBlockType -> -1 -> false
+          break;
+        }
+        if (pos + 80 > total_bits) {  // 4 CRC bytes follow either magic
+          set_err("bzip2: truncated CRC (Dart: RangeError)");
+          final_rc = B200Z_E_THROW;
+          break;
+        }
+        if (cand[ci] >> 63) {
+          have_eos[q] = 1;
+          eos_crc[q] = ccrc[ci];
+          break;  // end of stream: whatever follows is ignored (:83-84)
+        }
+        const uint32_t k = blk_of[ci];
+        if (h_st[k] == -2) {
+          set_err("bzip2: block at bit %llu reads past the end (Dart: RangeError)", (unsigned long long)pos);
+          final_rc = B200Z_E_THROW;
+          break;
+        }
+        if (h_st[k] != 0) {
+          set_err("bzip2: data error in the block at bit %llu", (unsigned long long)pos);
+          final_rc = B200Z_E_DATA;
+          break;
+        }
+        push_block(k, ccrc[ci]);
+        pos = h_end[k] - base_bit;
       }
-      if (mismatch) {
-        set_err("bzip2: no block signature at bit %llu", (unsigned long long)pos);
-        final_rc = B200Z_E_DATA;
-      } else {
-        set_err("bzip2: truncated block header (Dart: RangeError)");
-        final_rc = B200Z_E_THROW;
-      }
-      break;
+      s_rc[q] = final_rc;
+      if (getenv("B200Z_DEBUG"))
+        fprintf(stderr, "[b200z] bzip2: stream %zu: %u candidates, chain %zu, rc so far %d, eos %d\n", s, c_end - c_lo[s],
+                chain.size() - ch_lo[q], final_rc, (int)have_eos[q]);
     }
-    while (ci < ncand && (cand[ci] & ~(1ull << 63)) < pos) ++ci;
-    if (ci >= ncand || (cand[ci] & ~(1ull << 63)) != pos) {
-      set_err("bzip2: no block signature at bit %llu", (unsigned long long)pos);
-      final_rc = B200Z_E_DATA;  // _readBlockType -> -1 -> false
-      break;
-    }
-    if (pos + 80 > total_bits) {  // 4 CRC bytes follow either magic
-      set_err("bzip2: truncated CRC (Dart: RangeError)");
-      final_rc = B200Z_E_THROW;
-      break;
-    }
-    const uint32_t crc_field = be32_at_bit(in, in_len, pos + 48);
-    if (cand[ci] >> 63) {
-      have_eos = true;
-      eos_crc = crc_field;
-      break;  // end of stream: whatever follows is ignored (:83-84)
-    }
-    const uint32_t k = blk_of_cand[ci];
-    if (h_st[k] == -2) {
-      set_err("bzip2: block at bit %llu reads past the end (Dart: RangeError)", (unsigned long long)pos);
-      final_rc = B200Z_E_THROW;
-      break;
-    }
-    if (h_st[k] != 0) {
-      set_err("bzip2: data error in the block at bit %llu", (unsigned long long)pos);
-      final_rc = B200Z_E_DATA;
-      break;
-    }
-    chain.push_back({k, h_nblock[k], h_nrec[k], h_optr[k], h_rnd[k] ? 1u : 0u});  // randomised blocks: serial walk in K8
-    stored_crc.push_back(crc_field);
-    pos = h_end[k];
-  }
+    ch_lo[G] = (uint32_t)chain.size();
 
-  if (getenv("B200Z_DEBUG")) {
-    fprintf(stderr, "[b200z] bzip2: %u candidates (%u block), chain %zu, rc so far %d, eos %d\n", ncand, nb, chain.size(),
-            final_rc, (int)have_eos);
-    for (uint32_t i = 0; i < nb && i < 16; ++i)
-      fprintf(stderr, "[b200z]   cand %u bit %llu st %d nblock %u nrec %u optr %u end %llu\n", i,
-              (unsigned long long)blk_bits[i], h_st[i], h_nblock[i], h_nrec[i], h_optr[i], (unsigned long long)h_end[i]);
-  }
-  // ---- K8 on the chain ----
-  const uint32_t nc = (uint32_t)chain.size();
-  std::vector<unsigned long long> h_off(nc + 1, 0);
-  size_t early_copied = 0;  // bytes [0, early_copied) of the output are on their way to the host already (s_d2h)
-  std::vector<uint32_t> h_crc(nc);
-  std::vector<int32_t> h_irr(nc);
-  if (nc) {
-    CU(g.d_out.reserve(out_cap + 64));
-    CU(cudaMemcpyAsync(A.chain, chain.data(), (size_t)nc * sizeof(BzChainHost), cudaMemcpyHostToDevice, g.stream));
-    Bz2Ibwt w;
-    w.chain = A.chain; w.n_chain = nc; w.nblock_max = nblock_max;
-    w.rec_val = A.rec_val; w.rec_pos = A.rec_pos; w.sym8 = A.sym8; w.chist = A.chist; w.tt = A.tt;
-    w.seg_len = A.seg_len; w.seg_next = A.seg_next; w.seg_off = A.seg_off; w.seg_resume = A.seg_resume; w.slots = A.slots; w.walk_ctr = A.walk_ctr; w.irregular = A.irregular; w.cycle_len = A.cycle_len; w.raw = A.raw;
-    w.slice_state = A.slice_state; w.slice_out = A.slice_out; w.block_out = A.block_out; w.block_off = A.block_off;
-    w.block_crc = A.block_crc; w.out = (uint8_t *)g.d_out.p; w.out_cap = out_cap;
-    for (const BzChainHost &ce : chain) w.any_randomised = w.any_randomised || (ce.flags & 1u);
-    w.any_records = false;
-    for (const BzChainHost &ce : chain) w.any_records = w.any_records || ce.n_rec != 0;
-    // B200Z_BZ2_GROUPS=n decodes a long chain in n groups, the bytes of a finished group on their way to the host (copy
-    // stream) while the next group is decoded.  Measured slower than one piece (512 MiB, 597 blocks), and slower the
-    // more groups -- the pointer-chasing kernels of K8 are bound by latency, not by the number of blocks, so a group
-    // costs nearly what the whole chain costs.  Off by default.
-    uint32_t groups = 1u;
-    if (const char *ge = getenv("B200Z_BZ2_GROUPS")) groups = (uint32_t)std::max(1, atoi(ge));
-    if (shard || groups > nc) groups = 1;
-    // The RLE1 output pass (per block) runs in 4 groups and a finished group's bytes go to the host on
-    // the copy stream while the next group is written: the blocks' offsets are known before it, so nothing waits
-    // (B200Z_BZ2_EMIT_GROUPS, 1: one pass, one copy at the end).
-    uint32_t emit_groups = (!shard && nc >= 64) ? 4u : 1u;
-    if (const char *ge = getenv("B200Z_BZ2_EMIT_GROUPS")) emit_groups = (uint32_t)std::max(1, atoi(ge));
-    if (shard || emit_groups > nc || groups > 1) emit_groups = 1;
-    if (groups <= 1 && emit_groups > 1) {
-      w.phase = 1;
-      CU(bz2_launch_ibwt(w, g.stream));
-      CU(cudaMemcpyAsync(h_off.data(), A.block_off, (size_t)(nc + 1) * 8, cudaMemcpyDeviceToHost, g.stream));
-      CU(cudaStreamSynchronize(g.stream));
-      w.phase = 2;
-      for (uint32_t gi = 0; gi < emit_groups; ++gi) {
-        const uint32_t lo = (uint32_t)((uint64_t)nc * gi / emit_groups), hi = (uint32_t)((uint64_t)nc * (gi + 1) / emit_groups);
-        CU(bz2_launch_ibwt_group(w, lo, hi, g.stream));
-        cudaEvent_t ev;
-        CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        CU(cudaEventRecord(ev, g.stream));
-        CU(cudaStreamWaitEvent(g.s_d2h, ev, 0));
-        cudaEventDestroy(ev);  // (released once it has completed)
-        const size_t end = (size_t)(h_off[hi] < (unsigned long long)out_cap ? h_off[hi] : (unsigned long long)out_cap);
-        if (end > early_copied) {
-          CU(cudaMemcpyAsync(out + early_copied, (uint8_t *)g.d_out.p + early_copied, end - early_copied, cudaMemcpyDeviceToHost,
-                             g.s_d2h));
-          early_copied = end;
+    // ---- K8 on the chains of the group ----
+    const uint32_t nc = (uint32_t)chain.size();
+    std::vector<unsigned long long> h_off(nc + 1, 0), h_out(nc, 0);
+    std::vector<unsigned long long> early(s_lo);  // output bytes [s_lo, early) of each stream are on their way to the host (s_d2h)
+    bool any_early = false;
+    std::vector<uint32_t> h_crc(nc);
+    std::vector<int32_t> h_irr(nc);
+    // the bytes of the chain entries below `hi` are written: those in the streams' slots go to the host on the copy stream
+    auto copy_early = [&](uint32_t hi) -> int {
+      for (size_t q = 0; q < G; ++q) {
+        if (ch_lo[q] >= hi || ch_lo[q] == ch_lo[q + 1]) continue;
+        const uint32_t last = std::min(hi, ch_lo[q + 1]) - 1;
+        const unsigned long long end = std::min(h_off[last] + h_out[last], s_hi[q]);
+        if (end > early[q]) {
+          CU(cudaMemcpyAsync(jobs[grp[q]].out + (early[q] - s_lo[q]), (uint8_t *)g.d_out.p + early[q], end - early[q],
+                             cudaMemcpyDeviceToHost, g.s_d2h));
+          early[q] = end;
+          any_early = true;
         }
       }
-      w.phase = 0;
-    } else if (groups <= 1) {
-      CU(bz2_launch_ibwt(w, g.stream));
-    } else {
-      CU(g.h_meta.reserve((size_t)groups * 8));
-      volatile unsigned long long *h_end_off = (volatile unsigned long long *)g.h_meta.p;
-      std::vector<cudaEvent_t> ev(groups);
-      for (uint32_t gi = 0; gi < groups; ++gi) {
-        const uint32_t lo = (uint32_t)((uint64_t)nc * gi / groups), hi = (uint32_t)((uint64_t)nc * (gi + 1) / groups);
-        CU(bz2_launch_ibwt_group(w, lo, hi, g.stream));
-        CU(cudaMemcpyAsync((void *)(h_end_off + gi), A.block_off + hi, 8, cudaMemcpyDeviceToHost, g.stream));
-        CU(cudaEventCreateWithFlags(&ev[gi], cudaEventDisableTiming));
-        CU(cudaEventRecord(ev[gi], g.stream));
-      }
-      for (uint32_t gi = 0; gi < groups; ++gi) {
-        CU(cudaEventSynchronize(ev[gi]));
-        cudaEventDestroy(ev[gi]);
-        const unsigned long long eo = h_end_off[gi];
-        const size_t end = (size_t)(eo < (unsigned long long)out_cap ? eo : (unsigned long long)out_cap);
-        if (end > early_copied) {
-          CU(cudaMemcpyAsync(out + early_copied, (uint8_t *)g.d_out.p + early_copied, end - early_copied, cudaMemcpyDeviceToHost,
-                             g.s_d2h));
-          early_copied = end;
-        }
-      }
-    }
-    CU(cudaMemcpyAsync(h_off.data(), A.block_off, (size_t)(nc + 1) * 8, cudaMemcpyDeviceToHost, g.stream));
-    CU(cudaMemcpyAsync(h_crc.data(), A.block_crc, (size_t)nc * 4, cudaMemcpyDeviceToHost, g.stream));
-    CU(cudaMemcpyAsync(h_irr.data(), A.irregular, (size_t)nc * 4, cudaMemcpyDeviceToHost, g.stream));
-    CU(cudaStreamSynchronize(g.stream));
-    if (early_copied) CU(cudaStreamSynchronize(g.s_d2h));  // (no copy into the caller's buffer outlives this call)
-  }
-  if (getenv("B200Z_DEBUG"))
-    for (uint32_t i = 0; i < nc && i < 16; ++i)
-      fprintf(stderr, "[b200z]   chain %u off %llu..%llu crc %08x stored %08x irregular %d\n", i, (unsigned long long)h_off[i],
-              (unsigned long long)h_off[i + 1], h_crc[i], stored_crc[i], h_irr[i]);
-  if (shard) {
-    // one report per candidate of the range + one per end-of-stream candidate (every rank reports those)
-    shard->n_blocks = 0;
-    auto push = [&](const b200z_bz2_block &b) {
-      if (shard->n_blocks < shard->blocks_cap) shard->blocks[shard->n_blocks] = b;
-      shard->n_blocks++;
+      return B200Z_OK;
     };
-    for (uint32_t k = k_lo; k < k_hi; ++k) {
-      b200z_bz2_block b{};
-      b.start_bit = blk_bits[k];
-      b.end_bit = h_end[k];
-      b.status = h_st[k];
-      b.flags = 0u;  // randomised blocks are decoded like the others (serial walk)
-      b.crc_stored = blk_bits[k] + 80 <= total_bits ? be32_at_bit(in, in_len, blk_bits[k] + 48) : 0u;
-      const uint32_t c = chain_of[k];
-      if (c != 0xffffffffu) {
-        b.out_bytes = h_off[c + 1] - h_off[c];
-        b.crc_calc = h_crc[c];
-        if (h_irr[c] == 2) b.flags |= B200Z_BZ2_OVERRUN;
-        else if (h_irr[c]) b.flags |= B200Z_BZ2_CORRUPT_CYCLE;
+    if (nc) {
+      CU(g.d_out.reserve(dev_room + 64));
+      CU(cudaMemcpyAsync(A.chain, chain.data(), (size_t)nc * sizeof(BzChainHost), cudaMemcpyHostToDevice, g.stream));
+      Bz2Ibwt w;
+      w.chain = A.chain; w.n_chain = nc; w.nblock_max = stride;
+      w.rec_val = A.rec_val; w.rec_pos = A.rec_pos; w.sym8 = A.sym8; w.chist = A.chist; w.tt = A.tt;
+      w.seg_len = A.seg_len; w.seg_next = A.seg_next; w.seg_off = A.seg_off; w.seg_resume = A.seg_resume; w.slots = A.slots; w.walk_ctr = A.walk_ctr; w.irregular = A.irregular; w.cycle_len = A.cycle_len; w.raw = A.raw;
+      w.slice_state = A.slice_state; w.slice_out = A.slice_out; w.block_out = A.block_out; w.block_off = A.block_off;
+      w.block_crc = A.block_crc; w.out = (uint8_t *)g.d_out.p; w.out_cap = ~0ull;  // (each entry is clipped at its slot)
+      for (const BzChainHost &ce : chain) w.any_randomised = w.any_randomised || (ce.flags & 1u);
+      w.any_records = false;
+      for (const BzChainHost &ce : chain) w.any_records = w.any_records || ce.n_rec != 0;
+      // B200Z_BZ2_GROUPS=n decodes a long chain of one stream in n groups, the bytes of a finished group on their way to the
+      // host (copy stream) while the next group is decoded.  Measured slower than one piece (512 MiB, 597 blocks), and
+      // slower the more groups -- the pointer-chasing kernels of K8 are bound by latency, not by the number of blocks, so a
+      // group costs nearly what the whole chain costs.  Off by default.
+      uint32_t groups = 1u;
+      if (const char *ge = getenv("B200Z_BZ2_GROUPS")) groups = (uint32_t)std::max(1, atoi(ge));
+      if (shard || groups > nc || G > 1) groups = 1;
+      // The RLE1 output pass (per block) runs in 4 groups and a finished group's bytes go to the host on
+      // the copy stream while the next group is written: the blocks' offsets are known before it, so nothing waits
+      // (B200Z_BZ2_EMIT_GROUPS, 1: one pass, one copy at the end).
+      uint32_t emit_groups = (!shard && nc >= 64) ? 4u : 1u;
+      if (const char *ge = getenv("B200Z_BZ2_EMIT_GROUPS")) emit_groups = (uint32_t)std::max(1, atoi(ge));
+      if (shard || emit_groups > nc || groups > 1) emit_groups = 1;
+      if (groups <= 1 && emit_groups > 1) {
+        w.phase = 1;
+        CU(bz2_launch_ibwt(w, g.stream));
+        CU(cudaMemcpyAsync(h_off.data(), A.block_off, (size_t)(nc + 1) * 8, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaMemcpyAsync(h_out.data(), A.block_out, (size_t)nc * 8, cudaMemcpyDeviceToHost, g.stream));
+        CU(cudaStreamSynchronize(g.stream));
+        w.phase = 2;
+        for (uint32_t gi = 0; gi < emit_groups; ++gi) {
+          const uint32_t lo = (uint32_t)((uint64_t)nc * gi / emit_groups), hi = (uint32_t)((uint64_t)nc * (gi + 1) / emit_groups);
+          CU(bz2_launch_ibwt_group(w, lo, hi, g.stream));
+          cudaEvent_t ev;
+          CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+          CU(cudaEventRecord(ev, g.stream));
+          CU(cudaStreamWaitEvent(g.s_d2h, ev, 0));
+          cudaEventDestroy(ev);  // (released once it has completed)
+          const int rc = copy_early(hi);
+          if (rc) return rc;
+        }
+        w.phase = 0;
+      } else if (groups <= 1) {
+        CU(bz2_launch_ibwt(w, g.stream));
+      } else {  // (one stream: its slot starts at 0)
+        CU(g.h_meta.reserve((size_t)groups * 8));
+        volatile unsigned long long *h_end_off = (volatile unsigned long long *)g.h_meta.p;
+        std::vector<cudaEvent_t> ev(groups);
+        for (uint32_t gi = 0; gi < groups; ++gi) {
+          const uint32_t lo = (uint32_t)((uint64_t)nc * gi / groups), hi = (uint32_t)((uint64_t)nc * (gi + 1) / groups);
+          CU(bz2_launch_ibwt_group(w, lo, hi, g.stream));
+          CU(cudaMemcpyAsync((void *)(h_end_off + gi), A.block_off + hi, 8, cudaMemcpyDeviceToHost, g.stream));
+          CU(cudaEventCreateWithFlags(&ev[gi], cudaEventDisableTiming));
+          CU(cudaEventRecord(ev[gi], g.stream));
+        }
+        for (uint32_t gi = 0; gi < groups; ++gi) {
+          CU(cudaEventSynchronize(ev[gi]));
+          cudaEventDestroy(ev[gi]);
+          const unsigned long long end = std::min((unsigned long long)h_end_off[gi], s_hi[0]);
+          if (end > early[0]) {
+            CU(cudaMemcpyAsync(jobs[grp[0]].out + early[0], (uint8_t *)g.d_out.p + early[0], end - early[0], cudaMemcpyDeviceToHost,
+                               g.s_d2h));
+            early[0] = end;
+            any_early = true;
+          }
+        }
       }
-      push(b);
+      CU(cudaMemcpyAsync(h_off.data(), A.block_off, (size_t)(nc + 1) * 8, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaMemcpyAsync(h_out.data(), A.block_out, (size_t)nc * 8, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaMemcpyAsync(h_crc.data(), A.block_crc, (size_t)nc * 4, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaMemcpyAsync(h_irr.data(), A.irregular, (size_t)nc * 4, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaStreamSynchronize(g.stream));
+      if (any_early) CU(cudaStreamSynchronize(g.s_d2h));  // (no copy into the caller's buffer outlives this call)
     }
-    for (uint32_t i = 0; i < ncand; ++i)
-      if (cand[i] >> 63) {
+    if (shard) {
+      // one report per candidate of the range + one per end-of-stream candidate (every rank reports those)
+      Bz2Job &j = jobs[grp[0]];
+      const uint64_t total_bits = j.in_len * 8, base_bit = j.in_off * 8;
+      shard->n_blocks = 0;
+      auto push = [&](const b200z_bz2_block &b) {
+        if (shard->n_blocks < shard->blocks_cap) shard->blocks[shard->n_blocks] = b;
+        shard->n_blocks++;
+      };
+      for (uint32_t k = k_lo; k < k_hi; ++k) {
         b200z_bz2_block b{};
-        b.start_bit = cand[i] & ~(1ull << 63);
-        b.end_bit = b.start_bit + 80;
-        b.flags = B200Z_BZ2_EOS;
-        b.crc_stored = b.start_bit + 80 <= total_bits ? be32_at_bit(in, in_len, b.start_bit + 48) : 0u;
+        b.start_bit = blk_bits[k] - base_bit;
+        b.end_bit = h_end[k] - base_bit;
+        b.status = h_st[k];
+        b.flags = 0u;  // randomised blocks are decoded like the others (serial walk)
+        b.crc_stored = blk_crc[k];
+        const uint32_t c = chain_of[k];
+        if (c != 0xffffffffu) {
+          b.out_bytes = h_out[c];
+          b.crc_calc = h_crc[c];
+          if (h_irr[c] == 2) b.flags |= B200Z_BZ2_OVERRUN;
+          else if (h_irr[c]) b.flags |= B200Z_BZ2_CORRUPT_CYCLE;
+        }
         push(b);
       }
-    const size_t n_local = nc ? (size_t)h_off[nc] : 0;
-    *out_len = n_local;
-    if (shard->n_blocks > shard->blocks_cap) {
-      set_err("bzip2 shard: %zu block reports, capacity %zu", shard->n_blocks, shard->blocks_cap);
-      return B200Z_E_NOSPC;
+      for (uint32_t i = c_lo[grp[0]]; i < c_lo[grp[0] + 1]; ++i)
+        if (cand[i] >> 63) {
+          b200z_bz2_block b{};
+          b.start_bit = cand[i] & POS;
+          b.end_bit = b.start_bit + 80;
+          b.flags = B200Z_BZ2_EOS;
+          b.crc_stored = b.start_bit + 80 <= total_bits ? ccrc[i] : 0u;
+          push(b);
+        }
+      const size_t n_local = nc ? (size_t)(h_off[nc - 1] + h_out[nc - 1]) : 0;
+      j.out_len = n_local;
+      if (shard->n_blocks > shard->blocks_cap) {
+        set_err("bzip2 shard: %zu block reports, capacity %zu", shard->n_blocks, shard->blocks_cap);
+        j.rc = B200Z_E_NOSPC;
+      } else if (n_local > j.out_cap) {
+        set_err("bzip2 shard: output needs %zu bytes, out_cap %zu", n_local, j.out_cap);
+        j.rc = B200Z_E_NOSPC;
+      } else if (n_local) {
+        CU(cudaMemcpyAsync(j.out, g.d_out.p, n_local, cudaMemcpyDeviceToHost, g.stream));
+      }
+      CU(cudaStreamSynchronize(g.stream));
+      continue;
     }
-    if (n_local > out_cap) {
-      set_err("bzip2 shard: output needs %zu bytes, out_cap %zu", n_local, out_cap);
-      return B200Z_E_NOSPC;
+    // blocks are committed in order; the first bad one ends the stream (its bytes are already written when the
+    // reference compares the CRC, :58-66)
+    for (size_t q = 0; q < G; ++q) {
+      Bz2Job &j = jobs[grp[q]];
+      int final_rc = s_rc[q];
+      bool eos = have_eos[q] != 0;
+      size_t n_out = 0;
+      uint32_t combined = 0;
+      for (uint32_t i = ch_lo[q]; i < ch_lo[q + 1]; ++i) {
+        const uint32_t bi = i - ch_lo[q];
+        if (h_irr[i] == 1) {
+          set_err("bzip2: block %u: corrupt BWT cycle", bi);
+          final_rc = B200Z_E_DATA;
+          break;
+        }
+        n_out = (size_t)(h_off[i] + h_out[i] - s_lo[q]);
+        if (h_irr[i] == 2) {  // the run-length walk overran the block (:497-499, :628-631): false, its bytes are already written
+          set_err("bzip2: block %u: run overruns the block", bi);
+          final_rc = B200Z_E_DATA;
+          eos = false;
+          break;
+        }
+        if (verify && h_crc[i] != stored_crc[i]) {
+          set_err("bzip2: block %u CRC mismatch", bi);
+          final_rc = B200Z_E_DATA;
+          eos = false;
+          break;
+        }
+        combined = ((combined << 1) | (combined >> 31)) ^ h_crc[i];
+      }
+      if (final_rc == B200Z_OK && eos && verify && eos_crc[q] != combined) {
+        set_err("bzip2: combined CRC mismatch");
+        final_rc = B200Z_E_DATA;
+      }
+      j.out_len = n_out;
+      if (n_out > j.out_cap) {
+        set_err("bzip2: output needs %zu bytes, out_cap %zu", n_out, j.out_cap);
+        j.rc = B200Z_E_NOSPC;
+        continue;
+      }
+      j.rc = final_rc;
+      const size_t from = (size_t)(early[q] - s_lo[q]);
+      if (n_out > from)
+        CU(cudaMemcpyAsync(j.out + from, (uint8_t *)g.d_out.p + s_lo[q] + from, n_out - from, cudaMemcpyDeviceToHost, g.stream));
     }
-    if (n_local) CU(cudaMemcpyAsync(out, g.d_out.p, n_local, cudaMemcpyDeviceToHost, g.stream));
     CU(cudaStreamSynchronize(g.stream));
-    return B200Z_OK;
   }
-  // blocks are committed in order; the first bad one ends the stream (its bytes are already written when the
-  // reference compares the CRC, :58-66)
-  size_t n_out = 0;
-  uint32_t combined = 0;
-  for (uint32_t i = 0; i < nc; ++i) {
-    if (h_irr[i] == 1) {
-      set_err("bzip2: block %u: corrupt BWT cycle", i);
-      final_rc = B200Z_E_DATA;
-      break;
-    }
-    n_out = (size_t)h_off[i + 1];
-    if (h_irr[i] == 2) {  // the run-length walk overran the block (:497-499, :628-631): false, its bytes are already written
-      set_err("bzip2: block %u: run overruns the block", i);
-      final_rc = B200Z_E_DATA;
-      have_eos = false;
-      break;
-    }
-    if (verify && h_crc[i] != stored_crc[i]) {
-      set_err("bzip2: block %u CRC mismatch", i);
-      final_rc = B200Z_E_DATA;
-      have_eos = false;
-      break;
-    }
-    combined = ((combined << 1) | (combined >> 31)) ^ h_crc[i];
-  }
-  if (final_rc == B200Z_OK && have_eos && verify && eos_crc != combined) {
-    set_err("bzip2: combined CRC mismatch");
-    final_rc = B200Z_E_DATA;
-  }
-  *out_len = n_out;
-  if (n_out > out_cap) {
-    set_err("bzip2: output needs %zu bytes, out_cap %zu", n_out, out_cap);
-    return B200Z_E_NOSPC;
-  }
-  if (n_out > early_copied)
-    CU(cudaMemcpyAsync(out + early_copied, (uint8_t *)g.d_out.p + early_copied, n_out - early_copied, cudaMemcpyDeviceToHost,
-                       g.stream));
-  CU(cudaStreamSynchronize(g.stream));
-  return final_rc;
+  return B200Z_OK;
 }
 
 }  // namespace b200z
@@ -2346,9 +2502,8 @@ extern "C" int b200z_zip_comment(const uint8_t *z, size_t len, uint64_t *off, ui
 // Encrypted members after decryption (b200z_zip_extract_password): their plaintext sits in g.d_in behind the archive, and
 // the entries handed to zip_extract_core point there.
 struct ZipPlain {
-  size_t staged;                                // bytes of g.d_in in use: the archive, then the plaintext area
-  size_t archive_len;                           // of which the archive (the bytes the host holds)
-  const std::vector<const uint8_t *> *bz_src;   // per member: host copy of a decrypted bzip2 member, or null
+  size_t staged;       // bytes of g.d_in in use: the archive, then the plaintext area
+  size_t archive_len;  // of which the archive (the bytes the host holds)
 };
 
 // (test hooks) last b200z_zip_extract call's K12 batch: members offered, accepted, fell back, redo rounds, batches; kernel
@@ -2448,7 +2603,7 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
                             int32_t *status, uint32_t flags, const ZipPlain *pl) {
   int rc = B200Z_OK;
   // members: deflate -> one inflate batch; stored (and unknown methods, which the reference treats as stored,
-  // zip_file.dart:83) -> device copies; bzip2 -> one stream each, afterwards
+  // zip_file.dart:83) -> device copies; bzip2 -> one BZip2 batch, afterwards
   std::vector<uint64_t> u_in_off, u_out_off;
   std::vector<uint32_t> u_in_len, u_cap, u_idx;
   std::vector<size_t> bz_idx;
@@ -2498,7 +2653,7 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
     }
   }
   const bool any_dev = hi > lo;
-  if (any_dev || !u_idx.empty()) {
+  if (any_dev || !u_idx.empty() || !bz_idx.empty()) {
     if (!pl) {
       rc = stage_input(z, len);
       if (rc) return rc;
@@ -2650,13 +2805,20 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
     CU(cudaStreamSynchronize(g.stream));
     if (early_to > lo) CU(cudaStreamSynchronize(g.s_d2h));
   }
-  for (size_t i : bz_idx) {  // BZip2Decoder().decodeStream(_rawContent, output) (zip_file.dart:189-192,239-245)
-    const b200z_zip_entry &e = entries[i];
-    size_t got = 0;
-    const uint8_t *src = pl && (*pl->bz_src)[i] ? (*pl->bz_src)[i] : z + e.data_off;
-    rc = bzip2_decode_impl(src, (size_t)e.comp_size, 0, out + out_off[i], (size_t)out_room[i], &got);
-    out_len[i] = got;
-    status[i] = rc == B200Z_OK ? B200Z_U_DONE : rc == B200Z_E_NOSPC ? B200Z_U_NOSPC : rc == B200Z_E_THROW ? B200Z_U_THROW : B200Z_U_STOP;
+  if (!bz_idx.empty()) {  // BZip2Decoder().decodeStream(_rawContent, output) (zip_file.dart:189-192,239-245), all members at once
+    std::vector<Bz2Job> jobs(bz_idx.size());
+    for (size_t k = 0; k < bz_idx.size(); ++k) {
+      const size_t i = bz_idx[k];
+      jobs[k] = Bz2Job{entries[i].data_off, entries[i].comp_size, out + out_off[i], (size_t)out_room[i], 0, B200Z_OK};
+    }
+    rc = bzip2_decode_device((const uint8_t *)g.d_in.p, jobs.data(), jobs.size(), 0);
+    if (rc) return rc;
+    for (size_t k = 0; k < bz_idx.size(); ++k) {
+      const size_t i = bz_idx[k];
+      const int r = jobs[k].rc;
+      out_len[i] = jobs[k].out_len;
+      status[i] = r == B200Z_OK ? B200Z_U_DONE : r == B200Z_E_NOSPC ? B200Z_U_NOSPC : r == B200Z_E_THROW ? B200Z_U_THROW : B200Z_U_STOP;
+    }
   }
   return B200Z_OK;
 }
@@ -2886,24 +3048,14 @@ static int zip_extract_crypt(const uint8_t *z, size_t len, const b200z_zip_entry
     CU(cudaEventRecord(ev.ev[7], g.stream));
     ev.used[3] = true;
   }
-  // 5. bzip2 members are decoded from host memory (bzip2_decode_impl): their plaintext comes back first
-  std::vector<const uint8_t *> bz_src(n, nullptr);
-  std::vector<std::vector<uint8_t>> bz_keep;
-  for (size_t i = 0; i < n; ++i) {
-    if (!ve[i].has_data || !(entries[i].flags & 1u) || ve[i].method != 12 || ve[i].data_off < len) continue;
-    bz_keep.emplace_back(ve[i].comp_size + 1);
-    CU(cudaMemcpyAsync(bz_keep.back().data(), d_base + ve[i].data_off, ve[i].comp_size, cudaMemcpyDeviceToHost, g.stream));
-    bz_src[i] = bz_keep.back().data();
-  }
-  if (!bz_keep.empty()) CU(cudaStreamSynchronize(g.stream));
-  // 6. everything else sees the decrypted members as ranges of the staged buffer
-  const ZipPlain pl{staged, len, &bz_src};
+  // 5. every member kind sees the decrypted members as ranges of the staged buffer
+  const ZipPlain pl{staged, len};
   int rc = zip_extract_core(z, staged, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, &pl);
   if (rc) {
     cudaStreamSynchronize(s_mac);
     return rc;
   }
-  // 7. the MACs: HMAC-SHA1 of the ciphertext, first 10 bytes, against the 10 bytes that end the member
+  // 6. the MACs: HMAC-SHA1 of the ciphertext, first 10 bytes, against the 10 bytes that end the member
   if (na) {
     CU(cudaStreamSynchronize(s_mac));
     CU(cudaMemcpy(macs.data(), dc + cl.mac, na * 10, cudaMemcpyDeviceToHost));
@@ -3058,10 +3210,87 @@ int b200z_bzip2_decode(const uint8_t *in, size_t in_len, int verify, uint8_t *ou
   if (rc) return rc;
   std::lock_guard<std::mutex> lk(g.mu);
   CU(cudaSetDevice(g.device));
-  size_t n = 0;
-  rc = bzip2_decode_impl(in, in_len, verify, out, out_cap, &n);
-  if (out_len) *out_len = n;
-  return rc;
+  rc = stage_input(in, in_len);
+  if (rc) return rc;
+  CU(cudaMemsetAsync((uint8_t *)g.d_in.p + in_len, 0, 64, g.stream));
+  Bz2Job j{0, in_len, out, out_cap, 0, B200Z_OK};
+  rc = bzip2_decode_device((const uint8_t *)g.d_in.p, &j, 1, verify);
+  if (out_len) *out_len = j.out_len;
+  return rc ? rc : j.rc;
+}
+
+int b200z_bzip2_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                             uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  if (n && (!in_off || !in_len || !out_off || !out_cap || !out_len || !rc)) {
+    set_err("bzip2_decode_batch: null array");
+    return B200Z_E_ARG;
+  }
+  uint64_t lo = ~0ull, hi = 0, total = 0;
+  std::vector<size_t> by_out;
+  for (size_t i = 0; i < n; ++i) {
+    if (in_off[i] + in_len[i] < in_off[i] || out_off[i] + out_cap[i] < out_off[i] || (in_len[i] && !in_base) ||
+        (out_cap[i] && !out_base)) {
+      set_err("bzip2_decode_batch: stream %zu: bad range", i);
+      return B200Z_E_ARG;
+    }
+    if (in_len[i]) {
+      lo = std::min(lo, in_off[i]);
+      hi = std::max(hi, in_off[i] + in_len[i]);
+      total += in_len[i];
+    }
+    if (out_cap[i]) by_out.push_back(i);
+  }
+  std::sort(by_out.begin(), by_out.end(), [&](size_t a, size_t b) { return out_off[a] < out_off[b]; });
+  for (size_t k = 1; k < by_out.size(); ++k)
+    if (out_off[by_out[k - 1]] + out_cap[by_out[k - 1]] > out_off[by_out[k]]) {
+      set_err("bzip2_decode_batch: output slots %zu and %zu overlap", by_out[k - 1], by_out[k]);
+      return B200Z_E_ARG;
+    }
+  std::lock_guard<std::mutex> lk(g.mu);
+  if (n == 0) return bzip2_decode_device(nullptr, nullptr, 0, verify);
+  CU(cudaSetDevice(g.device));
+  // one copy to the device: the span of all inputs as it is, or the inputs packed when the span is mostly other bytes
+  std::vector<Bz2Job> jobs(n);
+  std::vector<uint8_t> packed;
+  const uint8_t *src = nullptr;
+  size_t staged = 0;
+  if (total == 0) {
+    for (size_t i = 0; i < n; ++i) jobs[i].in_off = 0;
+  } else if (hi - lo <= 2 * total + ((size_t)1 << 20)) {
+    src = in_base + lo;
+    staged = (size_t)(hi - lo);
+    for (size_t i = 0; i < n; ++i) jobs[i].in_off = in_len[i] ? in_off[i] - lo : 0;
+  } else {
+    packed.resize(total);
+    for (size_t i = 0; i < n; ++i) {
+      jobs[i].in_off = staged;
+      if (in_len[i]) memcpy(packed.data() + staged, in_base + in_off[i], in_len[i]);
+      staged += in_len[i];
+    }
+    src = packed.data();
+  }
+  r = stage_input(src, staged);
+  if (r) return r;
+  CU(cudaMemsetAsync((uint8_t *)g.d_in.p + staged, 0, 64, g.stream));
+  for (size_t i = 0; i < n; ++i) {
+    jobs[i].in_len = in_len[i];
+    jobs[i].out = out_base + out_off[i];
+    jobs[i].out_cap = out_cap[i];
+  }
+  r = bzip2_decode_device((const uint8_t *)g.d_in.p, jobs.data(), n, verify);
+  for (size_t i = 0; i < n; ++i) {
+    out_len[i] = jobs[i].out_len;
+    rc[i] = jobs[i].rc;
+  }
+  return r;
+}
+// (test hooks, not part of the ABI) cap on the blocks of one BZip2 device group (0: the memory budget alone); the last
+// b200z_bzip2_decode* or ZIP call's bzip2 streams, device groups and blocks
+void b200z_debug_bz2_batch_set(unsigned max_blocks) { g_bz2_max_group_blocks = max_blocks; }
+void b200z_debug_bz2_batch_stats(unsigned long long out[3]) {
+  for (int k = 0; k < 3; ++k) out[k] = g_bz2_stats[k];
 }
 void b200z_profile_enable(int on) { profile_enable(on != 0); }
 int b200z_crc32(const uint8_t *in, size_t in_len, uint32_t *crc) {
@@ -3119,11 +3348,14 @@ int b200z_bzip2_decode_shard(const uint8_t *in, size_t in_len, uint32_t rank, ui
   std::lock_guard<std::mutex> lk(g.mu);
   CU(cudaSetDevice(g.device));
   Bz2Shard sh{rank, world, blocks, blocks_cap, 0};
-  size_t n = 0;
-  rc = bzip2_decode_impl(in, in_len, 0, out, out_cap, &n, &sh);
-  if (out_len) *out_len = n;
+  rc = stage_input(in, in_len);
+  if (rc) return rc;
+  CU(cudaMemsetAsync((uint8_t *)g.d_in.p + in_len, 0, 64, g.stream));
+  Bz2Job j{0, in_len, out, out_cap, 0, B200Z_OK};
+  rc = bzip2_decode_device((const uint8_t *)g.d_in.p, &j, 1, 0, &sh);
+  if (out_len) *out_len = j.out_len;
   if (n_blocks) *n_blocks = sh.n_blocks;
-  return rc;
+  return rc ? rc : j.rc;
 }
 
 int b200z_bzip2_encode(const uint8_t *in, size_t in_len, uint8_t *out, size_t out_cap, size_t *out_len) {

@@ -82,6 +82,11 @@ struct Bz2Entropy {  // K7, one warp per candidate block
   int32_t *status;
   uint32_t *fast_flag = nullptr;  // [n_blocks], may be null: 1 = the block was decoded by k_bz2_entropy_fast
   uint8_t *sym8 = nullptr;        // [n_blocks][nblock_max]: K8's byte array, by candidate slot (the fast kernel writes it)
+  // [n_blocks], both may be null (every block then ends at n_bytes and has the limit nblock_max): the bit where the block's
+  // stream ends in `words` (reads from there on see zeros and are past the end) and its stream's level x 100000.  nblock_max
+  // stays the stride of the per-block arrays.
+  const unsigned long long *blk_end = nullptr;
+  const uint32_t *blk_lim = nullptr;
 };
 struct Bz2Ibwt {  // K8 over the validated chain
   const void *chain;  // BzChain[n_chain] (device)
@@ -109,11 +114,28 @@ struct Bz2Ibwt {  // K8 over the validated chain
 };
 struct BzChainHost {
   uint32_t cand, nblock, n_rec, orig_ptr;
-  uint32_t flags;  // bit 0: randomised block (serial path in K8)
+  uint32_t flags;  // bit 0: randomised block (serial path in K8); bit 1: first block of its stream (output starts at out_lo)
+  uint32_t pad_ = 0;
+  unsigned long long out_lo = 0, out_hi = ~0ull;  // the stream's output slot in Bz2Ibwt::out (clipped at out_cap as well)
+};
+struct Bz2ScanStream {
+  unsigned long long off, len;  // bytes of Bz2Scan::in
+};
+struct Bz2Scan {  // K6
+  const uint8_t *in = nullptr;
+  uint64_t n_bytes = 0;                            // without a stream table: one stream, in[0, n_bytes)
+  const Bz2ScanStream *streams = nullptr;          // [n_streams] (device), or null
+  const unsigned long long *first_thr = nullptr;   // [n_streams + 1]: first thread of each stream (4 bytes each, at least one)
+  uint32_t n_streams = 0;
+  unsigned long long *cand = nullptr;              // [cap]: bit in `in` | end-of-stream << 63
+  uint32_t *n_cand = nullptr, cap = 0;
+  uint32_t *cand_stream = nullptr, *cand_crc = nullptr;  // [cap], with a stream table: its stream, the 32 bits behind the magic
+  uint8_t *ends = nullptr;                         // [n_streams][12], with a stream table: first 4 and last 8 bytes (0 where none)
 };
 size_t bz2_entropy_smem();
 cudaError_t bz2_launch_scan(const uint8_t *d_in, uint64_t n_bytes, unsigned long long *d_cand, uint32_t *d_ncand,
                             uint32_t cap, cudaStream_t s);
+cudaError_t bz2_launch_scan_streams(const Bz2Scan &a, uint64_t n_threads, cudaStream_t s);
 cudaError_t bz2_launch_entropy(const Bz2Entropy &a, cudaStream_t s);
 // blocks K7 left with status -3 (a damaged block that the reference keeps decoding): d_list = their indices into a's arrays
 cudaError_t bz2_launch_entropy_literal(const Bz2Entropy &a, const uint32_t *d_list, uint32_t n_list, cudaStream_t s);

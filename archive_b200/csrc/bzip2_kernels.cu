@@ -38,17 +38,29 @@ struct BzBits {
   int cnt;             // valid bits in buf
   uint64_t next_word;  // index of the next word to load
   uint64_t n_words;    // words that contain stream bytes
+  uint32_t last_mask;  // bytes of word n_words - 1 that belong to the stream
+  // the stream's bytes end at bit end_bit of w: from there on the reader sees zeros, as behind a stream staged on its own,
+  // whatever bytes (another stream's) follow in the buffer
+  __device__ __forceinline__ void set_end(uint64_t end_bit) {
+    const uint64_t nb = end_bit >> 3;
+    n_words = (nb + 3) >> 2;
+    last_mask = (nb & 3) ? ~0u << (8 * (4 - (uint32_t)(nb & 3))) : ~0u;
+  }
+  __device__ __forceinline__ uint32_t word(uint64_t i) const {
+    const uint32_t v = i < n_words ? __byte_perm(__ldg(w + i), 0, 0x0123) : 0u;
+    return i + 1 == n_words ? v & last_mask : v;
+  }
   __device__ __forceinline__ void seek(uint64_t bitpos) {
     next_word = bitpos >> 5;
     uint32_t sh = (uint32_t)(bitpos & 31);
-    uint32_t v = next_word < n_words ? __byte_perm(__ldg(w + next_word), 0, 0x0123) : 0u;
+    uint32_t v = word(next_word);
     next_word++;
     buf = ((uint64_t)v << 32) << sh;
     cnt = 32 - (int)sh;
   }
   __device__ __forceinline__ void refill() {
     if (cnt <= 32) {
-      uint32_t v = next_word < n_words ? __byte_perm(__ldg(w + next_word), 0, 0x0123) : 0u;
+      uint32_t v = word(next_word);
       if ((next_word & 31u) == 0u) asm volatile("prefetch.global.L1 [%0];" ::"l"(w + next_word + 64));
       next_word++;
       buf |= (uint64_t)v << (32 - cnt);
@@ -67,14 +79,36 @@ struct BzBits {
 
 // ---------------------------------------------------------------------------------------------
 // K6: every bit offset is tested for the block magic 0x314159265359 and the end-of-stream magic
-// 0x177245385090 (bzip2.dart compressedMagic / eosMagic).  cand = bit position of the magic | type << 63.
+// 0x177245385090 (bzip2.dart compressedMagic / eosMagic).  cand = bit position of the magic in `in` | type << 63.
+// Over a stream table (a.streams) a magic counts only when it lies wholly inside its stream, each candidate carries its
+// stream and the 32 bits behind its magic (the stored CRC), and thread 0 of every stream copies the stream's first 4 and
+// last 8 bytes to a.ends (what the host needs of the header and of a truncated block signature).
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_bz2_scan(const uint8_t *__restrict__ in, uint64_t n_bytes,
-                                                  unsigned long long *__restrict__ cand, uint32_t *__restrict__ n_cand,
-                                                  uint32_t cap) {
+__global__ void __launch_bounds__(256) k_bz2_scan(const Bz2Scan a) {
   const uint64_t MAGIC_BLK = 0x314159265359ull, MAGIC_EOS = 0x177245385090ull;
-  uint64_t b0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t si = 0;
+  uint64_t off = 0, n_bytes = a.n_bytes, b0 = t * 4;
+  if (a.streams) {
+    if (t >= a.first_thr[a.n_streams]) return;
+    uint32_t lo = 0, hi = a.n_streams;  // the stream whose threads hold t: first_thr[lo] <= t < first_thr[lo + 1]
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (a.first_thr[mid] <= t) lo = mid;
+      else hi = mid;
+    }
+    si = lo;
+    off = a.streams[si].off;
+    n_bytes = a.streams[si].len;
+    b0 = (t - a.first_thr[si]) * 4;
+    if (b0 == 0 && a.ends) {
+      uint8_t *e = a.ends + (size_t)si * 12;
+      for (int i = 0; i < 4; ++i) e[i] = (uint64_t)i < n_bytes ? a.in[off + i] : 0;
+      for (int i = 0; i < 8; ++i) e[4 + i] = n_bytes + i >= 8 ? a.in[off + n_bytes + i - 8] : 0;
+    }
+  }
   if (b0 >= n_bytes) return;
+  const uint8_t *in = a.in + off;
   // 11 bytes cover 4 byte offsets x 8 bit shifts x 48 bits
   uint8_t by[12];
 #pragma unroll
@@ -92,8 +126,16 @@ __global__ void __launch_bounds__(256) k_bz2_scan(const uint8_t *__restrict__ in
       if (blk || eos) {
         uint64_t bit = (b0 + k) * 8 + s;
         if (bit + 48 <= n_bytes * 8) {
-          uint32_t slot = atomicAdd(n_cand, 1u);
-          if (slot < cap) cand[slot] = bit | (eos ? (1ull << 63) : 0ull);
+          uint32_t slot = atomicAdd(a.n_cand, 1u);
+          if (slot < a.cap) {
+            a.cand[slot] = (off * 8 + bit) | (eos ? (1ull << 63) : 0ull);
+            if (a.streams) {
+              uint64_t c = 0;  // (bytes past the stream's end read 0)
+              for (int i = 0; i < 5; ++i) c = (c << 8) | (b0 + k + 6 + i < n_bytes ? in[b0 + k + 6 + i] : 0);
+              a.cand_stream[slot] = si;
+              a.cand_crc[slot] = (uint32_t)(c >> (8 - s));
+            }
+          }
         }
       }
     }
@@ -275,21 +317,22 @@ k_bz2_entropy(const uint32_t *__restrict__ words, uint64_t n_bytes, const unsign
               uint32_t n_blocks, uint32_t nblock_max, uint32_t *__restrict__ rec_val, uint32_t *__restrict__ rec_pos,
               uint32_t *__restrict__ n_rec, uint32_t *__restrict__ nblock_out, uint32_t *__restrict__ orig_ptr,
               uint32_t *__restrict__ randomised, unsigned long long *__restrict__ end_bit, int32_t *__restrict__ status,
-              int only_redo) {
+              int only_redo, const unsigned long long *__restrict__ blk_end, const uint32_t *__restrict__ blk_lim) {
   extern __shared__ __align__(16) uint8_t smraw[];
   BzSmem &S = *reinterpret_cast<BzSmem *>(smraw);
   const uint32_t b = blockIdx.x;
   if (b >= n_blocks) return;
   if (only_redo && status[b] != -9) return;  // (BZ_REDO) the fast kernel has decoded this block
   const int lane = threadIdx.x;
-  const uint64_t total_bits = n_bytes * 8;
+  const uint64_t total_bits = blk_end ? blk_end[b] : n_bytes * 8;
+  const uint32_t lim = blk_lim ? blk_lim[b] : nblock_max;  // the block's own limit; nblock_max is the stride of its arrays
   __shared__ int s_groups, s_alpha, s_err, s_nsel, s_inuse;
   __shared__ uint32_t s_optr, s_rnd;
   __shared__ unsigned long long s_bitpos;
 
   BzBits br;
   br.w = words;
-  br.n_words = (n_bytes + 3) >> 2;
+  br.set_end(total_bits);
   int err = 0;
   uint32_t rnd = 0, optr = 0;
   int n_groups = 0, n_sel = 0, alpha = 0, n_in_use = 0;
@@ -419,7 +462,7 @@ k_bz2_entropy(const uint32_t *__restrict__ words, uint64_t n_bytes, const unsign
         run_n++;
       } else {
         if (run_n) {
-          if (nblock + run_es > nblock_max) {  // (:313-316)
+          if (nblock + run_es > lim) {  // (:313-316)
             err = BZ_DATA;
             break;
           }
@@ -429,7 +472,7 @@ k_bz2_entropy(const uint32_t *__restrict__ words, uint64_t n_bytes, const unsign
           run_es = 0;
         }
         if (sym == eob) break;
-        if (nblock >= nblock_max) {  // (:326-329)
+        if (nblock >= lim) {  // (:326-329)
           err = BZ_DATA;
           break;
         }
@@ -544,18 +587,24 @@ k_bz2_entropy_fast(const uint32_t *__restrict__ words, uint64_t n_bytes, const u
                    uint32_t n_blocks, uint32_t nblock_max, uint32_t *__restrict__ rec_val, uint32_t *__restrict__ rec_pos,
                    uint32_t *__restrict__ n_rec, uint32_t *__restrict__ nblock_out, uint32_t *__restrict__ orig_ptr,
                    uint32_t *__restrict__ randomised, unsigned long long *__restrict__ end_bit, int32_t *__restrict__ status,
-                   uint32_t *__restrict__ fast_flag, uint8_t *__restrict__ sym8) {
+                   uint32_t *__restrict__ fast_flag, uint8_t *__restrict__ sym8, const unsigned long long *__restrict__ blk_end,
+                   const uint32_t *__restrict__ blk_lim) {
   __shared__ BzFast S;
   const uint32_t b = blockIdx.x;
   if (b >= n_blocks) return;
   if (fast_flag && threadIdx.x == 0) fast_flag[b] = 0;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const unsigned FULLW = 0xffffffffu;
-  const uint64_t total_bits = n_bytes * 8, n_words = (n_bytes + 3) >> 2;
+  const uint64_t total_bits = blk_end ? blk_end[b] : n_bytes * 8;
+  const uint32_t lim = blk_lim ? blk_lim[b] : nblock_max;  // the block's own limit; nblock_max is the stride of its arrays
+  // The walker and the decoder read whole words up to the stream's end without masking the bytes that follow it (another
+  // stream's, in a batch): a block is only accepted here when all its symbols end inside the stream, and those symbols
+  // do not depend on what follows; a block that reads further is handed to the exact kernel, whose reader sees zeros.
+  const uint64_t n_words = ((total_bits >> 3) + 3) >> 2;
   if (tid == 0) {
     BzBits br;
     br.w = words;
-    br.n_words = n_words;
+    br.set_end(total_bits);
     BzHdr h;
     bz_parse_header(S, br, blk_bit[b], total_bits, h);
     S.hdr = h;
@@ -811,7 +860,7 @@ k_bz2_entropy_fast(const uint32_t *__restrict__ words, uint64_t n_bytes, const u
           const unsigned LR = __ballot_sync(FULLW, longrun);
           if (isnr) {
             const uint32_t pos_sym = st_nblock + st_v + pa + (uint32_t)__popc(below);
-            if (pos_sym >= nblock_max) {  // (:313-316, :326-329)
+            if (pos_sym >= lim) {  // (:313-316, :326-329)
               lbad = true;
             } else {
               if (hasrun) {
@@ -843,7 +892,7 @@ k_bz2_entropy_fast(const uint32_t *__restrict__ words, uint64_t n_bytes, const u
           }
         }
         if (lastb && st_n) {  // the run that the end-of-block code closes (:306-321)
-          if (st_n > 21u || st_nblock + st_v > nblock_max) {
+          if (st_n > 21u || st_nblock + st_v > lim) {
             lbad = true;
           } else if (st_v > BZF_INLINE_RUN) {
             if (lane == 0) {
@@ -913,14 +962,16 @@ __global__ void __launch_bounds__(32)
 k_bz2_entropy_literal(const uint32_t *__restrict__ words, uint64_t n_bytes, const unsigned long long *__restrict__ blk_bit,
                       const uint32_t *__restrict__ list, uint32_t n_list, uint32_t nblock_max, uint32_t *__restrict__ rec_val,
                       uint32_t *__restrict__ rec_pos, uint32_t *__restrict__ n_rec, uint32_t *__restrict__ nblock_out,
-                      unsigned long long *__restrict__ end_bit, int32_t *__restrict__ status) {
+                      unsigned long long *__restrict__ end_bit, int32_t *__restrict__ status,
+                      const unsigned long long *__restrict__ blk_end, const uint32_t *__restrict__ blk_lim) {
   __shared__ BzLitSmem S;
   if (blockIdx.x >= n_list || threadIdx.x != 0) return;
   const uint32_t b = list[blockIdx.x];
-  const uint64_t total_bits = n_bytes * 8;
+  const uint64_t total_bits = blk_end ? blk_end[b] : n_bytes * 8;
+  const uint32_t lim = blk_lim ? blk_lim[b] : nblock_max;  // the block's own limit; nblock_max is the stride of its arrays
   BzBits br;
   br.w = words;
-  br.n_words = (n_bytes + 3) >> 2;
+  br.set_end(total_bits);
   br.seek(blk_bit[b] + 48 + 32 + 1);  // the randomised bit is K7's to report
   uint32_t optr = br.get(8);
   optr = (optr << 8) | br.get(8);
@@ -1067,7 +1118,7 @@ k_bz2_entropy_literal(const uint32_t *__restrict__ words, uint64_t n_bytes, cons
         if (err) break;
         if (br.bitpos() > total_bits) continue;  // -> BZ_THROW at the top
         es++;
-        if ((long long)nblock + es > (long long)nblock_max) {  // (:313-316): fills up to the limit, then -1
+        if ((long long)nblock + es > (long long)lim) {  // (:313-316): fills up to the limit, then -1
           err = BZ_DATA;
           break;
         }
@@ -1077,7 +1128,7 @@ k_bz2_entropy_literal(const uint32_t *__restrict__ words, uint64_t n_bytes, cons
         nblock += (uint32_t)es;
         continue;
       }
-      if (nblock >= nblock_max) {
+      if (nblock >= lim) {
         err = BZ_DATA;
         break;
       }
@@ -1136,7 +1187,9 @@ struct BzChain {           // one entry per block that is on the validated chain
   uint32_t nblock;
   uint32_t n_rec;
   uint32_t orig_ptr;
-  uint32_t flags;          // bit 0: randomised block
+  uint32_t flags;          // bit 0: randomised block; bit 1: first block of its stream (its output starts at out_lo)
+  uint32_t pad_;
+  unsigned long long out_lo, out_hi;  // the stream's output slot [out_lo, out_hi) in `out` (bytes from out_hi on are dropped)
 };
 
 __global__ void __launch_bounds__(256)
@@ -1534,12 +1587,13 @@ k_bz2_rle_count(const BzChain *__restrict__ chain, const uint8_t *__restrict__ r
   }
 }
 
-// exclusive scan of the block sizes (a few hundred values)
-__global__ void k_bz2_offsets(const unsigned long long *__restrict__ block_out, uint32_t n_chain,
+// exclusive scan of the block sizes (a few thousand values), started again at its slot by the first block of every stream
+__global__ void k_bz2_offsets(const BzChain *__restrict__ chain, const unsigned long long *__restrict__ block_out, uint32_t n_chain,
                               unsigned long long *__restrict__ block_off, int carry) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     unsigned long long run = carry ? block_off[0] : 0;  // (a later group of the chain goes on where the one before it ended)
     for (uint32_t i = 0; i < n_chain; ++i) {
+      if (chain[i].flags & 2u) run = chain[i].out_lo;
       block_off[i] = run;
       run += block_out[i];
     }
@@ -1558,6 +1612,7 @@ k_bz2_rle_emit(const BzChain *__restrict__ chain, const uint8_t *__restrict__ ra
   __shared__ uint32_t sm_len[BZ_RLE_THREADS];
   const BzChain c = chain[blockIdx.x];
   if (c.flags & 1u) return;  // randomised: k_bz2_rand
+  if (c.out_hi < out_cap) out_cap = c.out_hi;
   const uint32_t t = threadIdx.x;
   if (t < 256) {
     uint32_t v = t << 24;
@@ -1660,6 +1715,7 @@ __global__ void k_bz2_rand(const BzChain *__restrict__ chain, uint32_t n_chain, 
   if (i >= n_chain) return;
   const BzChain c = chain[i];
   if (!(c.flags & 1u) || c.nblock == 0) return;
+  if (c.out_hi < out_cap) out_cap = c.out_hi;
   const uint8_t *src = raw + (size_t)i * nblock_max;
   const uint32_t nb = c.nblock;
   const uint32_t cl = cycle_len[i] ? cycle_len[i] : nb;  // the walk goes round a cycle of cl <= nblock bytes (k_bz2_walk_order)
@@ -1751,16 +1807,25 @@ __global__ void k_bz2_rand(const BzChain *__restrict__ chain, uint32_t n_chain, 
 // ---------------------------------------------------------------------------------------------
 size_t bz2_entropy_smem() { return sizeof(BzSmem); }
 
-cudaError_t bz2_launch_scan(const uint8_t *d_in, uint64_t n_bytes, unsigned long long *d_cand, uint32_t *d_ncand, uint32_t cap,
-                            cudaStream_t s) {
-  cudaError_t e = cudaMemsetAsync(d_ncand, 0, 4, s);
+cudaError_t bz2_launch_scan_streams(const Bz2Scan &a, uint64_t n_threads, cudaStream_t s) {
+  cudaError_t e = cudaMemsetAsync(a.n_cand, 0, 4, s);
   if (e != cudaSuccess) return e;
-  uint64_t threads = (n_bytes + 3) / 4;
-  unsigned blocks = (unsigned)((threads + 255) / 256);
+  const uint64_t blocks = (n_threads + 255) / 256;
   if (blocks == 0) return cudaSuccess;
-  k_bz2_scan<<<blocks, 256, 0, s>>>(d_in, n_bytes, d_cand, d_ncand, cap);
+  k_bz2_scan<<<(unsigned)blocks, 256, 0, s>>>(a);
   count_launch();
   return cudaGetLastError();
+}
+
+cudaError_t bz2_launch_scan(const uint8_t *d_in, uint64_t n_bytes, unsigned long long *d_cand, uint32_t *d_ncand, uint32_t cap,
+                            cudaStream_t s) {
+  Bz2Scan a;
+  a.in = d_in;
+  a.n_bytes = n_bytes;
+  a.cand = d_cand;
+  a.n_cand = d_ncand;
+  a.cap = cap;
+  return bz2_launch_scan_streams(a, (n_bytes + 3) / 4, s);
 }
 
 cudaError_t bz2_launch_entropy(const Bz2Entropy &a, cudaStream_t s) {
@@ -1778,12 +1843,12 @@ cudaError_t bz2_launch_entropy(const Bz2Entropy &a, cudaStream_t s) {
   if (fast) {
     k_bz2_entropy_fast<<<a.n_blocks, BZF_NT, 0, s>>>(a.words, a.n_bytes, a.blk_bit, a.n_blocks, a.nblock_max, a.rec_val, a.rec_pos,
                                                  a.n_rec, a.nblock, a.orig_ptr, a.randomised, a.end_bit, a.status,
-                                                 a.fast_flag, a.sym8);
+                                                 a.fast_flag, a.sym8, a.blk_end, a.blk_lim);
     count_launch();
   }
   k_bz2_entropy<<<a.n_blocks, 32, sizeof(BzSmem), s>>>(a.words, a.n_bytes, a.blk_bit, a.n_blocks, a.nblock_max, a.rec_val,
                                                        a.rec_pos, a.n_rec, a.nblock, a.orig_ptr, a.randomised, a.end_bit,
-                                                       a.status, fast);
+                                                       a.status, fast, a.blk_end, a.blk_lim);
   count_launch();
   return cudaGetLastError();
 }
@@ -1791,7 +1856,7 @@ cudaError_t bz2_launch_entropy(const Bz2Entropy &a, cudaStream_t s) {
 cudaError_t bz2_launch_entropy_literal(const Bz2Entropy &a, const uint32_t *d_list, uint32_t n_list, cudaStream_t s) {
   if (n_list == 0) return cudaSuccess;
   k_bz2_entropy_literal<<<n_list, 32, 0, s>>>(a.words, a.n_bytes, a.blk_bit, d_list, n_list, a.nblock_max, a.rec_val, a.rec_pos,
-                                              a.n_rec, a.nblock, a.end_bit, a.status);
+                                              a.n_rec, a.nblock, a.end_bit, a.status, a.blk_end, a.blk_lim);
   count_launch();
   return cudaGetLastError();
 }
@@ -1838,7 +1903,7 @@ cudaError_t bz2_launch_ibwt(const Bz2Ibwt &a, cudaStream_t s) {
                                                            a.out_cap, a.out, a.block_crc, a.irregular, a.cycle_len);
     count_launch();
   }
-  k_bz2_offsets<<<1, 32, 0, s>>>(a.block_out, a.n_chain, a.block_off, a.carry_off ? 1 : 0);
+  k_bz2_offsets<<<1, 32, 0, s>>>(chain, a.block_out, a.n_chain, a.block_off, a.carry_off ? 1 : 0);
   count_launch();
   }
   if (a.phase == 1) return cudaGetLastError();

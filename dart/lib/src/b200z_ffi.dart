@@ -39,6 +39,10 @@ typedef _Bz2DecodeC = Int32 Function(
     Pointer<Uint8> inp, Size inLen, Int32 verify, Pointer<Uint8> out, Size outCap, Pointer<Size> outLen);
 typedef _Bz2DecodeD = int Function(
     Pointer<Uint8> inp, int inLen, int verify, Pointer<Uint8> out, int outCap, Pointer<Size> outLen);
+typedef _Bz2DecodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Int32 verify, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Int32> rc);
+typedef _Bz2DecodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    int verify, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Int32> rc);
 
 typedef _DeflateRawC = Int32 Function(Pointer<Uint8> inp, Size inLen, Int32 level, Int32 windowBits, Pointer<Uint8> out,
     Size outCap, Pointer<Size> outLen, Pointer<Uint32> crc32OfInput);
@@ -229,6 +233,8 @@ class B200Z {
   late final _ZlibDecodeD zlibDecode = _lib.lookupFunction<_ZlibDecodeC, _ZlibDecodeD>('b200z_zlib_decode');
   late final _BoundD gzipBound = _lib.lookupFunction<_BoundC, _BoundD>('b200z_gzip_bound');
   late final _Bz2DecodeD bzip2Decode = _lib.lookupFunction<_Bz2DecodeC, _Bz2DecodeD>('b200z_bzip2_decode');
+  late final _Bz2DecodeBatchD bzip2DecodeBatch =
+      _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_bzip2_decode_batch');
   late final _DeflateRawD deflateRaw = _lib.lookupFunction<_DeflateRawC, _DeflateRawD>('b200z_deflate_raw');
   late final _SizeOfD deflateBound = _lib.lookupFunction<_SizeOfC, _SizeOfD>('b200z_deflate_bound');
   late final _ZlibEncodeD zlibEncode = _lib.lookupFunction<_ZlibEncodeC, _ZlibEncodeD>('b200z_zlib_encode');

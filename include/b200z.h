@@ -114,6 +114,16 @@ int b200z_gzip_encode(const uint8_t *in, size_t in_len, int level, uint32_t mtim
  * before the failure are kept, as in the reference).                                                    */
 int b200z_bzip2_decode(const uint8_t *in, size_t in_len, int verify, uint8_t *out, size_t out_cap,
                        size_t *out_len);
+/* n independent BZip2Decoder().decodeBytes(data, verify:) calls in one.  Stream i reads in_base[in_off[i] .. +in_len[i])
+ * and writes out_base[out_off[i] .. +out_cap[i]); rc[i] and out_len[i] are exactly what b200z_bzip2_decode returns and
+ * reports for that stream alone (B200Z_OK / _E_DATA / _E_THROW / _E_NOSPC), and so are the bytes in its slot (up to
+ * out_len[i]; after B200Z_E_NOSPC the slot's contents are unspecified, as after a single call).  The call
+ * returns B200Z_OK unless an argument is wrong or the device fails; n == 0 is OK.  Input ranges may overlap or repeat;
+ * output slots must not overlap.  All inputs go to the device in one copy, one scan finds the blocks of all streams, and
+ * the streams share the entropy and inverse-BWT launches (in groups that fit the device memory).                     */
+int b200z_bzip2_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                             uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                             int32_t *rc);
 /* One rank's share of a BZip2 stream (SURVEY.md 8e: blocks are independent once the bit-level magic scan has found
  * them; only the combined CRC and the output offsets chain across blocks).  Rank `rank` of `world` decodes the block
  * candidates [n*rank/world, n*(rank+1)/world) into `out`, back to back, and reports EVERY candidate of its share plus
@@ -167,9 +177,9 @@ int b200z_crc64(const uint8_t *in, size_t in_len, uint64_t *crc);
  * b200z_zip_list   = ZipDirectory.read (zip_directory.dart:25-183) + ZipFileHeader.read (zip_file_header.dart:28-111)
  *                    + ZipFile.read (zip_file.dart:73-149), host only: no device is needed.
  * b200z_zip_extract = ZipFile.getStream / decompress (zip_file.dart:164-249) for ALL listed members at once: the deflate
- *                    members are one batch of the inflate kernels, stored members are copies, bzip2 members are
- *                    decoded one after the other.  Names are byte ranges of the archive (decoding them is the host
- *                    language's business).  Encrypted members (ZipCrypto / AES) are reported, not decoded, unless a
+ *                    members are one batch of the inflate kernels, stored members are copies, the bzip2 members
+ *                    are one BZip2 batch (b200z_bzip2_decode_batch) on the staged archive.  Names are byte ranges of
+ *                    the archive (decoding them is the host language's business).  Encrypted members (ZipCrypto / AES) are reported, not decoded, unless a
  *                    password is given (b200z_zip_extract_password).                                                    */
 typedef struct {
   uint64_t local_header_off; /* ZipFileHeader.localHeaderOffset (zip64 applied)                               */

@@ -98,6 +98,8 @@ _SIGS = {
                                            C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_bzip2_encode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_bzip2_bound": (C.c_size_t, [C.c_size_t]),
+    "b200z_bzip2_encode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_file_codec": (C.c_int, [C.c_int, C.c_char_p, C.c_uint64, C.c_uint64, C.c_char_p, C.c_uint64, C.c_int32, C.c_int32,
                                    C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "b200z_file_last_stats": (None, [C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),

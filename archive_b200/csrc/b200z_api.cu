@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -3189,10 +3190,145 @@ extern "C" void b200z_debug_zip_chunked_stats(unsigned long long out[5], double 
   for (int k = 0; k < 5; ++k) out[k] = g_zck_stats[k];
   for (int k = 0; k < 3; ++k) ms[k] = g_zck_ms[k];
 }
-// (test hook) cap on the blocks b200z_bzip2_encode sorts and codes in one batch (0: the built-in plan), so that inputs of a
-// few blocks run through several batches
-static uint32_t g_bz2e_max_batch = 0;
+// (test hooks) cap on the blocks b200z_bzip2_encode / _encode_batch sort and code in one batch (0: the built-in plan), so
+// that inputs of a few blocks run through several batches; cap on the streams of one device group (0: the memory budget
+// alone); the last encode call's streams, device groups, block batches, blocks and serially sorted blocks
+static uint32_t g_bz2e_max_batch = 0, g_bz2e_max_group = 0;
+static unsigned long long g_bz2e_stats[5] = {0, 0, 0, 0, 0};
 extern "C" void b200z_debug_bzip2_encode_batch_set(unsigned max_batch) { g_bz2e_max_batch = max_batch; }
+extern "C" void b200z_debug_bzip2_encode_group_set(unsigned max_streams) { g_bz2e_max_group = max_streams; }
+extern "C" void b200z_debug_bzip2_encode_batch_stats(unsigned long long out[5]) {
+  for (int k = 0; k < 5; ++k) out[k] = g_bz2e_stats[k];
+}
+
+// n BZip2 encodes (arguments checked, g.mu held).  Consecutive streams form device groups that fit the memory budget
+// and keep staged positions below 4 GiB; each group is one multi-stream pass of the encoder (bz2e::encode_streams).
+static int bzip2_encode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                                uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                                uint32_t *crc32, int32_t *rc) {
+  const uint64_t kTile = 4096, kMaxIn = 0xfff00000ull;
+  for (int k = 0; k < 5; ++k) g_bz2e_stats[k] = 0;
+  g_bz2e_stats[0] = n;
+  std::vector<size_t> todo;
+  for (size_t i = 0; i < n; ++i) {
+    out_len[i] = 0;
+    if (crc32) crc32[i] = 0;
+    if (in_len[i] >= kMaxIn) {
+      set_err("bzip2 encode: inputs of 4 GiB and more are not supported");
+      rc[i] = B200Z_E_ARG;
+    } else {
+      todo.push_back(i);
+    }
+  }
+  if (todo.empty()) return B200Z_OK;
+  CU(cudaSetDevice(g.device));
+  size_t free_b = 0, total_b = 0;
+  CU(cudaMemGetInfo(&free_b, &total_b));
+  size_t budget = free_b + g.d_ws.cap > ((size_t)2 << 30) ? (free_b + g.d_ws.cap) / 2 : ((size_t)1 << 30);
+  if (budget > ((size_t)24 << 30)) budget = (size_t)24 << 30;
+  auto slot_of = [](uint64_t len) { return (uint64_t)align_up(bz2e::bound(len) + 64, 256); };
+  for (size_t k = 0; k < todo.size();) {
+    // the group [k, e): the first stream always, then while input, slots and workspace fit
+    bz2e::PlanSums sums;
+    bz2e::Plan plan{};
+    uint64_t staged = 0, slots = 0;
+    size_t e = k;
+    for (; e < todo.size(); ++e) {
+      const uint64_t len = in_len[todo[e]];
+      bz2e::PlanSums t = sums;
+      bz2e::plan_add(t, len);
+      const uint64_t st2 = staged + align_up(len, kTile), sl2 = slots + slot_of(len);
+      const bz2e::Plan p2 = bz2e::plan_of(t, budget);
+      if (e > k && (st2 > kMaxIn || (g_bz2e_max_group && e - k >= g_bz2e_max_group) || st2 + sl2 + p2.ws_bytes > budget))
+        break;
+      sums = t;
+      staged = st2;
+      slots = sl2;
+      plan = p2;
+    }
+    if (g_bz2e_max_batch && g_bz2e_max_batch < plan.batch) plan.batch = g_bz2e_max_batch;
+    const size_t m = e - k;
+    // layout: every stream starts on a 4 KiB tile, in stream order
+    std::vector<bz2e::StreamDesc> sd(m);
+    uint64_t in0 = 0, out0 = 0, in_end = 0, out_end = 0;
+    uint32_t blk0 = 0;
+    bool as_is = true;  // the inputs already lie so in the caller's buffer: stage the span as it is
+    uint64_t lo = ~0ull;
+    for (size_t j = 0; j < m; ++j) {
+      const size_t i = todo[k + j];
+      const uint64_t len = in_len[i];
+      sd[j] = bz2e::StreamDesc{(uint32_t)in0, (uint32_t)len, (uint32_t)(in0 / kTile), bz2e::tiles_of(len), blk0,
+                               bz2e::max_blocks_of(len), out0, slot_of(len)};
+      if (len) {
+        if (lo == ~0ull) lo = in_off[i];
+        if (in_off[i] != lo + in0) as_is = false;
+        in_end = in0 + len;
+      }
+      in0 += align_up(len, kTile);
+      blk0 += sd[j].max_blocks;
+      out0 += sd[j].out_cap;
+    }
+    out_end = out0;
+    std::unique_ptr<uint8_t[]> packed;
+    const uint8_t *src = nullptr;
+    if (in_end && as_is) {
+      src = in_base + lo;
+    } else if (in_end) {
+      packed.reset(new uint8_t[in_end]);
+      for (size_t j = 0; j < m; ++j)
+        if (sd[j].n) memcpy(packed.get() + sd[j].in0, in_base + in_off[todo[k + j]], sd[j].n);
+      src = packed.get();
+    }
+    int r = stage_input(src, in_end);
+    if (r) return r;
+    CU(g.d_out.reserve(out_end));
+    CU(g.d_ws.reserve(plan.ws_bytes));
+    std::vector<unsigned long long> lens(m);
+    std::vector<uint32_t> tile_crc(crc32 ? plan.n_tiles : 0);
+    bz2e::Stats st{0, 0, 0, 0, 0};
+    r = bz2e::encode_streams((const uint8_t *)g.d_in.p, sd.data(), (uint8_t *)g.d_out.p, g.d_ws.p, plan, lens.data(),
+                             crc32 ? tile_crc.data() : nullptr, &st, (void *)g.stream);
+    if (r == -3) {
+      set_err("bzip2 encode: internal output bound too small");
+      return B200Z_E_INTERNAL;
+    }
+    if (r != 0) {
+      cudaError_t ce = cudaGetLastError();
+      set_err("bzip2 encode: device failure (%s)", cudaGetErrorString(ce));
+      return B200Z_E_INTERNAL;
+    }
+    g_bz2e_stats[1]++;
+    g_bz2e_stats[2] += st.n_batches;
+    g_bz2e_stats[3] += st.n_blocks;
+    g_bz2e_stats[4] += st.n_serial_blocks;
+    // the outputs: one copy back, then each stream to its slot
+    const uint64_t used = sd[m - 1].out0 + lens[m - 1];
+    for (size_t j = 0; j < m; ++j) {
+      const size_t i = todo[k + j];
+      out_len[i] = lens[j];
+      if (crc32) crc32[i] = bz2e::crc32_fold(tile_crc.data() + sd[j].tile0, sd[j].n);
+      rc[i] = lens[j] > out_cap[i] ? B200Z_E_NOSPC : B200Z_OK;
+      if (rc[i] == B200Z_E_NOSPC)
+        set_err("bzip2 encode: output needs %llu bytes, out_cap %llu", (unsigned long long)lens[j],
+                (unsigned long long)out_cap[i]);
+    }
+    if (m == 1) {
+      if (rc[todo[k]] == B200Z_OK)
+        CU(cudaMemcpyAsync(out_base + out_off[todo[k]], g.d_out.p, lens[0], cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaStreamSynchronize(g.stream));
+    } else {
+      std::unique_ptr<uint8_t[]> h_out(new uint8_t[used]);
+      CU(cudaMemcpyAsync(h_out.get(), g.d_out.p, used, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaStreamSynchronize(g.stream));
+      for (size_t j = 0; j < m; ++j) {
+        const size_t i = todo[k + j];
+        if (rc[i] == B200Z_OK && lens[j]) memcpy(out_base + out_off[i], h_out.get() + sd[j].out0, lens[j]);
+      }
+    }
+    k = e;
+  }
+  return B200Z_OK;
+}
 
 extern "C" {
 
@@ -3366,38 +3502,41 @@ int b200z_bzip2_encode(const uint8_t *in, size_t in_len, uint8_t *out, size_t ou
     return B200Z_E_ARG;
   }
   std::lock_guard<std::mutex> lk(g.mu);
-  CU(cudaSetDevice(g.device));
-  rc = stage_input(in, in_len);
+  const uint64_t off = 0, len = in_len, cap = out_cap;
+  uint64_t n = 0;
+  int32_t r1 = B200Z_OK;
+  rc = bzip2_encode_streams(in, &off, &len, 1, out, &off, &cap, &n, nullptr, &r1);
   if (rc) return rc;
-  size_t free_b = 0, total_b = 0;
-  CU(cudaMemGetInfo(&free_b, &total_b));
-  const size_t budget = free_b + g.d_ws.cap > ((size_t)2 << 30) ? (free_b + g.d_ws.cap) / 2 : ((size_t)1 << 30);
-  bz2e::Plan plan = bz2e::plan(in_len, budget < ((size_t)24 << 30) ? budget : ((size_t)24 << 30));
-  if (g_bz2e_max_batch && g_bz2e_max_batch < plan.batch) plan.batch = g_bz2e_max_batch;
-  const size_t cap = align_up(bz2e::bound(in_len) + 64, 256);
-  CU(g.d_out.reserve(cap));
-  CU(g.d_ws.reserve(plan.ws_bytes));
-  size_t n = 0;
-  bz2e::Stats st;
-  int r = bz2e::encode_device((const uint8_t *)g.d_in.p, in_len, (uint8_t *)g.d_out.p, cap, g.d_ws.p, plan, &n, &st,
-                              (void *)g.stream);
-  if (r == -3) {
-    set_err("bzip2 encode: internal output bound too small (%zu)", cap);
-    return B200Z_E_INTERNAL;
+  if (out_len) *out_len = (size_t)n;
+  return r1;
+}
+
+int b200z_bzip2_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                             uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                             uint32_t *crc32, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  if (n && (!in_off || !in_len || !out_off || !out_cap || !out_len || !rc)) {
+    set_err("bzip2_encode_batch: null array");
+    return B200Z_E_ARG;
   }
-  if (r != 0) {
-    cudaError_t e = cudaGetLastError();
-    set_err("bzip2 encode: device failure (%s)", cudaGetErrorString(e));
-    return B200Z_E_INTERNAL;
+  std::vector<size_t> by_out;
+  for (size_t i = 0; i < n; ++i) {
+    if (in_off[i] + in_len[i] < in_off[i] || out_off[i] + out_cap[i] < out_off[i] || (in_len[i] && !in_base) ||
+        (out_cap[i] && !out_base)) {
+      set_err("bzip2_encode_batch: stream %zu: bad range", i);
+      return B200Z_E_ARG;
+    }
+    if (out_cap[i]) by_out.push_back(i);
   }
-  if (out_len) *out_len = n;
-  if (n > out_cap) {
-    set_err("bzip2 encode: output needs %zu bytes, out_cap %zu", n, out_cap);
-    return B200Z_E_NOSPC;
-  }
-  CU(cudaMemcpyAsync(out, g.d_out.p, n, cudaMemcpyDeviceToHost, g.stream));
-  CU(cudaStreamSynchronize(g.stream));
-  return B200Z_OK;
+  std::sort(by_out.begin(), by_out.end(), [&](size_t a, size_t b) { return out_off[a] < out_off[b]; });
+  for (size_t k = 1; k < by_out.size(); ++k)
+    if (out_off[by_out[k - 1]] + out_cap[by_out[k - 1]] > out_off[by_out[k]]) {
+      set_err("bzip2_encode_batch: output slots %zu and %zu overlap", by_out[k - 1], by_out[k]);
+      return B200Z_E_ARG;
+    }
+  std::lock_guard<std::mutex> lk(g.mu);
+  return bzip2_encode_streams(in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, crc32, rc);
 }
 size_t b200z_bzip2_bound(size_t in_len) { return bz2e::bound(in_len); }
 

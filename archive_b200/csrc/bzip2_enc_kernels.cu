@@ -56,13 +56,28 @@ constexpr uint32_t NET = 451;              // ceil(900 000 / 2000) + 1
 __device__ __forceinline__ uint32_t emit_of(uint32_t cl) { return cl < 4 ? cl : 5u; }
 
 // ---------------------------------------------------------------------------------------------
-// A1: per input tile, the length of its leading and trailing run
+// A1: per input tile, the end of its stream and the length of its leading and trailing run.  Every stream starts on a
+// tile, so no tile holds bytes of two streams.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-k_e_tile_info(const uint8_t *__restrict__ in, uint32_t n, uint32_t *__restrict__ t_head, uint32_t *__restrict__ t_tail) {
-  __shared__ uint32_t s_min, s_max;
+k_e_tile_info(const uint8_t *__restrict__ in, const StreamDesc *__restrict__ sd, uint32_t n_streams,
+              uint32_t *__restrict__ t_end, uint32_t *__restrict__ t_head, uint32_t *__restrict__ t_tail) {
+  __shared__ uint32_t s_min, s_max, s_n;
   const uint32_t tile = blockIdx.x, t = threadIdx.x;
   const uint32_t base = tile * TI;
+  if (t == 0) {
+    // the last stream whose first tile is at or before this one: an empty stream has no tile, so it is never the answer
+    uint32_t lo = 0, hi = n_streams;
+    while (hi - lo > 1) {
+      uint32_t mid = (lo + hi) >> 1;
+      if (sd[mid].tile0 <= tile) lo = mid;
+      else hi = mid;
+    }
+    s_n = sd[lo].in0 + sd[lo].n;
+    t_end[tile] = s_n;
+  }
+  __syncthreads();
+  const uint32_t n = s_n;
   const uint32_t len = umin(TI, n - base);
   if (t == 0) {
     s_min = len;
@@ -87,10 +102,11 @@ k_e_tile_info(const uint8_t *__restrict__ in, uint32_t n, uint32_t *__restrict__
   }
 }
 
-// A2: pre[t] = number of bytes immediately before tile t that equal its first byte (a segmented sum over tiles)
+// A2: pre[t] = number of bytes immediately before tile t, in its stream, that equal its first byte (a segmented sum over
+// tiles that restarts at every stream's first tile)
 __global__ void __launch_bounds__(1024)
 k_e_tile_pre(const uint8_t *__restrict__ in, uint32_t nt, const uint32_t *__restrict__ t_head,
-             const uint32_t *__restrict__ t_tail, uint32_t *__restrict__ pre) {
+             const uint32_t *__restrict__ t_tail, const uint32_t *__restrict__ t_end, uint32_t *__restrict__ pre) {
   __shared__ uint32_t s_p[1024], s_v[1024];
   const uint32_t t = threadIdx.x;
   const uint32_t per = (nt + 1023) / 1024;
@@ -98,7 +114,7 @@ k_e_tile_pre(const uint8_t *__restrict__ in, uint32_t nt, const uint32_t *__rest
   // element k (1 <= k < nt): pre[k] = p ? pre[k-1] + v : v
   uint32_t P = 1, V = 0;
   for (uint32_t k = lo; k < hi; ++k) {
-    bool conn = in[(size_t)k * TI - 1] == in[(size_t)k * TI];
+    bool conn = t_end[k - 1] == t_end[k] && in[(size_t)k * TI - 1] == in[(size_t)k * TI];
     bool uni = t_head[k - 1] == TI;
     uint32_t p = conn && uni, v = conn ? (uni ? TI : t_tail[k - 1]) : 0u;
     if (p) V += v;
@@ -122,7 +138,7 @@ k_e_tile_pre(const uint8_t *__restrict__ in, uint32_t nt, const uint32_t *__rest
   uint32_t run = s_v[t];
   if (t == 0) pre[0] = 0;
   for (uint32_t k = lo; k < hi; ++k) {
-    bool conn = in[(size_t)k * TI - 1] == in[(size_t)k * TI];
+    bool conn = t_end[k - 1] == t_end[k] && in[(size_t)k * TI - 1] == in[(size_t)k * TI];
     bool uni = t_head[k - 1] == TI;
     run = conn ? (uni ? run + TI : t_tail[k - 1]) : 0u;
     pre[k] = run;
@@ -136,7 +152,7 @@ k_e_tile_pre(const uint8_t *__restrict__ in, uint32_t nt, const uint32_t *__rest
 // ---------------------------------------------------------------------------------------------
 template <bool FILL>
 __global__ void __launch_bounds__(256)
-k_e_tile_emit(const uint8_t *__restrict__ in, uint32_t n, uint32_t tile0, const uint32_t *__restrict__ pre,
+k_e_tile_emit(const uint8_t *__restrict__ in, const uint32_t *__restrict__ t_end, uint32_t tile0, const uint32_t *__restrict__ pre,
               uint32_t *__restrict__ t_sum, uint16_t *__restrict__ sub_sum, uint32_t *__restrict__ sub_pre,
               const unsigned long long *__restrict__ G, const BlkInfo *__restrict__ blk, uint32_t blk_lo, uint32_t blk_hi,
               uint8_t *__restrict__ blockbuf, uint32_t *__restrict__ inuse) {
@@ -146,6 +162,7 @@ k_e_tile_emit(const uint8_t *__restrict__ in, uint32_t n, uint32_t tile0, const 
   __shared__ uint32_t s_use[2][8];
   const uint32_t tile = tile0 + blockIdx.x, t = threadIdx.x;
   const uint32_t base = tile * TI;
+  const uint32_t n = t_end[tile];  // end of the tile's stream: no run reaches past it
   const uint32_t len = umin(TI, n - base);
   const uint32_t i0 = t * 16;
   uint8_t by[18];  // by[0] = byte before the range, by[1..16] = the range, by[17] = byte after
@@ -284,7 +301,8 @@ k_scan_u32_u64(const uint32_t *__restrict__ in, uint32_t n, unsigned long long *
 }
 
 // ---------------------------------------------------------------------------------------------
-// A5: the block cuts (one warp; every lane runs the same scalar code, only the two searches are lane-parallel)
+// A5: the block cuts (one warp per stream; every lane runs the same scalar code, only the two searches are lane-parallel).
+// The context is the stream alone: positions from its first byte, its tiles, so no search reads past its last byte.
 // ---------------------------------------------------------------------------------------------
 struct CutCtx {
   const uint8_t *in;
@@ -342,12 +360,21 @@ __device__ uint32_t run_end(const CutCtx &c, uint32_t s) {
 }
 
 __global__ void __launch_bounds__(32)
-k_e_cut(const uint8_t *__restrict__ in, uint32_t n, uint32_t nt, const uint16_t *__restrict__ sub_sum,
-        const uint32_t *__restrict__ sub_pre, const unsigned long long *__restrict__ G, BlkInfo *__restrict__ blk,
-        uint32_t max_blocks, uint32_t *__restrict__ n_blocks) {
+k_e_cut(const uint8_t *__restrict__ in_all, const StreamDesc *__restrict__ sd, const uint16_t *__restrict__ sub_sum_all,
+        const uint32_t *__restrict__ sub_pre_all, const unsigned long long *__restrict__ G_all, BlkInfo *__restrict__ blk_all,
+        uint32_t *__restrict__ n_blocks_all) {
+  const uint32_t si = blockIdx.x;
+  const StreamDesc d = sd[si];
+  const uint8_t *in = in_all + d.in0;
+  const uint32_t n = d.n, nt = d.n_tiles, max_blocks = d.max_blocks;
+  const uint16_t *sub_sum = sub_sum_all + (size_t)d.tile0 * SUBS;
+  const uint32_t *sub_pre = sub_pre_all + (size_t)d.tile0 * SUBS;
+  const unsigned long long *G = G_all + d.tile0;
+  BlkInfo *blk = blk_all + d.blk0;
+  uint32_t *n_blocks = n_blocks_all + 2 * si;
   CutCtx c{in, n, nt, sub_sum, sub_pre, G};
   const uint32_t lane = threadIdx.x & 31;
-  const unsigned long long gtot = G[nt];
+  const unsigned long long gtot = n ? G[nt] : 0;
   uint32_t b = 0, s = 0;
   while (s < n && b < max_blocks) {
     const uint32_t e0 = run_end(c, s);
@@ -410,13 +437,15 @@ k_e_cut(const uint8_t *__restrict__ in, uint32_t n, uint32_t nt, const uint16_t 
     const uint32_t end = cpos < n ? cpos + 1 : n;
     if (lane == 0) {
       BlkInfo bi;
-      bi.start = s;
-      bi.end = end;
-      bi.e0 = e0u;
-      bi.c = cpos;
+      bi.start = d.in0 + s;
+      bi.end = d.in0 + end;
+      bi.e0 = d.in0 + e0u;
+      bi.c = d.in0 + cpos;
       bi.A = A;
       bi.nblock = F + (cpos < n ? 1u : 0u);
       bi.gx0 = gx0;
+      bi.stream = si;
+      bi.send = d.in0 + n;
       blk[b] = bi;
     }
     s = end;
@@ -430,7 +459,7 @@ k_e_cut(const uint8_t *__restrict__ in, uint32_t n, uint32_t nt, const uint16_t 
 
 // A7: the first run of every block (chopped from the block start, not from the start of the run) + the closing byte
 __global__ void __launch_bounds__(256)
-k_e_fill_head(const uint8_t *__restrict__ in, uint32_t n, const BlkInfo *__restrict__ blk, uint32_t blk_lo,
+k_e_fill_head(const uint8_t *__restrict__ in, const BlkInfo *__restrict__ blk, uint32_t blk_lo,
               uint8_t *__restrict__ blockbuf, uint32_t *__restrict__ inuse) {
   const uint32_t bl = blockIdx.y;
   const BlkInfo bi = blk[blk_lo + bl];
@@ -452,7 +481,7 @@ k_e_fill_head(const uint8_t *__restrict__ in, uint32_t n, const BlkInfo *__restr
     atomicOr(&u[ch >> 5], 1u << (ch & 31));
     if (full > 0) atomicOr(&u[251 >> 5], 1u << (251 & 31));
     if (rem >= 4) atomicOr(&u[(rem - 4) >> 5], 1u << ((rem - 4) & 31));
-    if (bi.c < n) {
+    if (bi.c < bi.send) {
       uint8_t p = in[bi.c];
       dst[bi.nblock - 1] = p;
       atomicOr(&u[p >> 5], 1u << (p & 31));
@@ -536,6 +565,34 @@ __global__ void k_e_crc_final(const uint32_t *__restrict__ part_crc, const uint3
   }
   uint32_t r = bzcrc_mulmod(0xffffffffu, bzcrc_xpow8(len)) ^ crc;
   block_crc[bl] = r ^ 0xffffffffu;
+}
+
+// A9: CRC-32 (reflected 0xEDB88320, as zlib's crc32) of every input tile, one thread each; crc32_fold joins a stream's
+__global__ void __launch_bounds__(256)
+k_e_crc32_tiles(const uint8_t *__restrict__ in, const uint32_t *__restrict__ t_end, uint32_t nt, uint32_t *__restrict__ tile_crc) {
+  __shared__ uint32_t tab[256];
+  {
+    uint32_t c = threadIdx.x;
+    for (int k = 0; k < 8; ++k) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+    tab[threadIdx.x] = c;
+  }
+  __syncthreads();
+  const uint32_t tile = blockIdx.x * 256 + threadIdx.x;
+  if (tile >= nt) return;
+  const uint32_t base = tile * TI, len = umin(TI, t_end[tile] - base);
+  uint32_t c = 0xffffffffu;
+  uint32_t i = 0;
+  if (len == TI) {  // tiles start at 4 KiB offsets of the staged input, so whole tiles read as 16-byte words
+    const uint4 *w4 = (const uint4 *)(in + base);
+    for (; i < TI; i += 16) {
+      const uint4 v = w4[i / 16];
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+      for (int k = 0; k < 4; ++k)
+        for (int b = 0; b < 4; ++b) c = tab[(c ^ (w[k] >> (8 * b))) & 0xffu] ^ (c >> 8);
+    }
+  }
+  for (; i < len; ++i) c = tab[(c ^ in[base + i]) & 0xffu] ^ (c >> 8);
+  tile_crc[tile] = c ^ 0xffffffffu;
 }
 
 #include "bzip2_enc_sort.inl"

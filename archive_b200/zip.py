@@ -268,6 +268,34 @@ def deflate_batch(contents, level: int = 6, window_bits: int = 15):
     return [(out[int(out_off[i]):int(out_off[i] + out_len[i])].tobytes(), int(crc[i])) for i in range(n)]
 
 
+def bzip2_encode_batch(contents):
+    """BZip2 of every item of `contents` with ONE b200z_bzip2_encode_batch call (all inputs staged at once, blocks of
+    different items sorted and coded together) -> list of (payload, crc32).  Each payload equals
+    BZip2Encoder().encodeBytes(item); crc32 is getCrc32(item), computed on the device."""
+    import numpy as np
+    L = _ffi.ensure_init()
+    n = len(contents)
+    if n == 0:
+        return []
+    in_len = np.array([len(c) for c in contents], dtype=np.uint64)
+    in_off = np.zeros(n, dtype=np.uint64)
+    in_off[1:] = np.cumsum(in_len)[:-1]
+    blob = b"".join(bytes(c) for c in contents)
+    addr, nb, keep = _ffi.as_buffer(blob if blob else b"\0")
+    out_cap = np.array([L.b200z_bzip2_bound(int(x)) for x in in_len], dtype=np.uint64)
+    out_off = np.zeros(n, dtype=np.uint64)
+    out_off[1:] = np.cumsum(out_cap)[:-1]
+    out = np.empty(int(out_cap.sum()), dtype=np.uint8)
+    out_len = np.zeros(n, dtype=np.uint64)
+    crc = np.zeros(n, dtype=np.uint32)
+    status = np.zeros(n, dtype=np.int32)
+    p = lambda a: a.ctypes.data
+    _ffi.check(L.b200z_bzip2_encode_batch(addr, p(in_off), p(in_len), n, p(out), p(out_off), p(out_cap), p(out_len),
+                                          p(crc), p(status)))
+    assert not status.any(), "b200z_bzip2_bound is an upper bound"
+    return [(out[int(out_off[i]):int(out_off[i] + out_len[i])].tobytes(), int(crc[i])) for i in range(n)]
+
+
 def aes_encrypt_batch(payloads, salts, password: bytes):
     """ZipEncoder._encryptCompressedData (zip_encoder.dart:166-183) for every payload at once: ONE b200z_zip_aes_encrypt call
     (key derivation, AES-256-CTR and the MAC on the device) -> list of (ciphertext, verifier, mac)."""
@@ -305,8 +333,9 @@ class ZipEncoder:
     VERSION = 20
 
     def __init__(self, compress=None, batch: bool = False, password=None, salt=None, encrypt=None):
-        """batch=True: all deflate members go to the device in one b200z_deflate_batch call (several members in flight)
-        instead of one b200z_deflate_raw call each; the archive bytes are the same.  password: str or bytes (see
+        """batch=True: all deflate members go to the device in one b200z_deflate_batch call per level (several members in
+        flight) instead of one b200z_deflate_raw call each, and all bzip2 members in one b200z_bzip2_encode_batch call;
+        the archive bytes are the same.  password: str or bytes (see
         password_bytes); salt: callable returning each member's 16 salt bytes (default os.urandom, as Random.secure);
         encrypt: stand-in for aes_encrypt_batch (the CPU test tier)."""
         import os
@@ -333,10 +362,12 @@ class ZipEncoder:
             for lv in sorted({level_of(archive[i]) for i in idx}):  # one device batch per level in use
                 grp = [i for i in idx if level_of(archive[i]) == lv]
                 table.update(zip(grp, deflate_batch([archive[i].content or b"" for i in grp], lv)))
+            grp = [i for i, e in enumerate(archive) if e.is_file and e.compression == "bzip2"]
+            table.update(zip(grp, bzip2_encode_batch([archive[i].content or b"" for i in grp])))
             at = [None]
 
             def compress(content, method, level_):
-                return table[at[0]] if method == "deflate" else self._compress(content, method, level_)
+                return table[at[0]] if method in ("deflate", "bzip2") else self._compress(content, method, level_)
         pw = self._password
         payloads = []
         for pos_in_archive, entry in enumerate(archive):

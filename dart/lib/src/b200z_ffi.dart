@@ -43,6 +43,12 @@ typedef _Bz2DecodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64>
     Int32 verify, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Int32> rc);
 typedef _Bz2DecodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
     int verify, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Int32> rc);
+typedef _Bz2EncodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Uint32> crc32,
+    Pointer<Int32> rc);
+typedef _Bz2EncodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Uint32> crc32,
+    Pointer<Int32> rc);
 
 typedef _DeflateRawC = Int32 Function(Pointer<Uint8> inp, Size inLen, Int32 level, Int32 windowBits, Pointer<Uint8> out,
     Size outCap, Pointer<Size> outLen, Pointer<Uint32> crc32OfInput);
@@ -240,6 +246,8 @@ class B200Z {
   late final _ZlibEncodeD zlibEncode = _lib.lookupFunction<_ZlibEncodeC, _ZlibEncodeD>('b200z_zlib_encode');
   late final _GzipEncodeD gzipEncode = _lib.lookupFunction<_GzipEncodeC, _GzipEncodeD>('b200z_gzip_encode');
   late final _Bz2EncodeD bzip2Encode = _lib.lookupFunction<_Bz2EncodeC, _Bz2EncodeD>('b200z_bzip2_encode');
+  late final _Bz2EncodeBatchD bzip2EncodeBatch =
+      _lib.lookupFunction<_Bz2EncodeBatchC, _Bz2EncodeBatchD>('b200z_bzip2_encode_batch');
   late final _SizeOfD bzip2Bound = _lib.lookupFunction<_SizeOfC, _SizeOfD>('b200z_bzip2_bound');
   late final _FileCodecD fileCodec = _lib.lookupFunction<_FileCodecC, _FileCodecD>('b200z_file_codec');
   late final _ZipListD zipList = _lib.lookupFunction<_ZipListC, _ZipListD>('b200z_zip_list');

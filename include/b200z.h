@@ -150,6 +150,18 @@ int b200z_bzip2_decode_shard(const uint8_t *in, size_t in_len, uint32_t rank, ui
  * Inputs of 4 GiB and more: B200Z_E_ARG.                                                                       */
 int b200z_bzip2_encode(const uint8_t *in, size_t in_len, uint8_t *out, size_t out_cap, size_t *out_len);
 size_t b200z_bzip2_bound(size_t in_len); /* output capacity that always suffices */
+/* n independent BZip2Encoder().encodeBytes(data) calls in one.  Stream i reads in_base[in_off[i] .. +in_len[i]) and
+ * writes out_base[out_off[i] .. +out_cap[i]); rc[i], out_len[i] and the bytes in its slot are exactly what
+ * b200z_bzip2_encode gives for that stream alone: B200Z_OK, B200Z_E_NOSPC (out_len[i] = the size needed, the slot's
+ * contents unspecified) or B200Z_E_ARG for a stream of 4 GiB or more (the others are still encoded).  crc32 may be
+ * NULL; otherwise crc32[i] = getCrc32 of stream i's input (crc32.dart, as b200z_crc32), computed on the device.  The
+ * call returns B200Z_OK unless an argument is wrong (null arrays, wrapping ranges, overlapping output slots: nothing
+ * is written) or the device fails; n == 0 is OK.  Input ranges may overlap or repeat.  All inputs go to the device in
+ * one copy, and blocks of different streams share the sort, MTF and entropy launches (in groups that fit the device
+ * memory).                                                                                                        */
+int b200z_bzip2_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                             uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                             uint32_t *crc32, int32_t *rc);
 
 /* getCrc32(bytes) -- crc32.dart:6-27 (CRC-32, reflected 0xEDB88320) of a host buffer, computed on the device (tile CRCs
  * folded with x^(8n) mod P): what ZipEncoder stores for members it does not deflate (zip_encoder.dart:113-134).   */

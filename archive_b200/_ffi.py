@@ -84,6 +84,10 @@ _SIGS = {
     "b200z_xz_encode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_xz_encode_bound": (C.c_size_t, [C.c_size_t]),
     "b200z_crc64": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]),
+    "b200z_xz_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_xz_encode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_zip_list": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_zip_comment": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     "b200z_zip_extract": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,

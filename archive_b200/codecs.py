@@ -349,6 +349,76 @@ def get_crc64(data) -> int:
     return crc.value
 
 
+def _pack(items):
+    """bytes-likes -> (ctypes buffer holding them back to back, in_off array, in_len array)."""
+    views = [memoryview(s).cast("B") for s in items]
+    n = len(views)
+    in_off = (C.c_uint64 * n)()
+    in_len = (C.c_uint64 * n)()
+    pos = 0
+    for i, v in enumerate(views):
+        in_off[i], in_len[i] = pos, len(v)
+        pos += len(v)
+    buf = (C.c_uint8 * max(pos, 1))()
+    for i, v in enumerate(views):
+        C.memmove(C.addressof(buf) + in_off[i], bytes(v), len(v))
+    return buf, in_off, in_len
+
+
+def _slots(sizes):
+    n = len(sizes)
+    out_off = (C.c_uint64 * n)()
+    cap = (C.c_uint64 * n)(*sizes)
+    total = 0
+    for i in range(n):
+        out_off[i] = total
+        total += sizes[i]
+    return (C.c_uint8 * max(total, 1))(), out_off, cap
+
+
+def xz_decode_batch(streams, verify: bool = False) -> list:
+    """XZDecoder().decodeBytes(stream, verify:) for every stream of `streams` in one b200z_xz_decode_batch call: a list of
+    (rc, bytes) in the same order.  rc is what b200z_xz_decode gives for that stream alone: OK, E_DATA (decodeStream
+    returned false; bytes = what was written before it) or E_THROW (the reference throws a RangeError; bytes = the output
+    before the chunk that throws).  Each output room is b200z_xz_bound of its stream, which always suffices."""
+    L = _ffi.ensure_init()
+    n = len(streams)
+    if n == 0:
+        return []
+    in_buf, in_off, in_len = _pack(streams)
+    base = C.addressof(in_buf)
+    out, out_off, cap = _slots([L.b200z_xz_bound(base + in_off[i], in_len[i]) for i in range(n)])
+    out_len = (C.c_uint64 * n)()
+    rc = (C.c_int32 * n)()
+    _ffi.check(L.b200z_xz_decode_batch(base, in_off, in_len, n, int(verify), C.addressof(out), out_off, cap, out_len, rc))
+    result = []
+    for i in range(n):
+        if rc[i] not in (_ffi.OK, _ffi.E_DATA, _ffi.E_THROW):
+            _ffi.check(rc[i])
+        result.append((rc[i], C.string_at(C.addressof(out) + out_off[i], out_len[i])))
+    return result
+
+
+def xz_encode_batch(contents, check: int = XZCheck.crc64) -> list:
+    """XZEncoder().encodeBytes(data, check:) for every input of `contents` in one b200z_xz_encode_batch call: the list of
+    encoded streams in the same order, each identical to what XZEncoder gives for that input alone."""
+    L = _ffi.ensure_init()
+    n = len(contents)
+    if n == 0:
+        return []
+    in_buf, in_off, in_len = _pack(contents)
+    out, out_off, cap = _slots([L.b200z_xz_encode_bound(in_len[i]) for i in range(n)])
+    out_len = (C.c_uint64 * n)()
+    rc = (C.c_int32 * n)()
+    _ffi.check(L.b200z_xz_encode_batch(C.addressof(in_buf), in_off, in_len, n, int(check), C.addressof(out), out_off, cap,
+                                       out_len, rc))
+    result = []
+    for i in range(n):
+        _ffi.check(rc[i])
+        result.append(C.string_at(C.addressof(out) + out_off[i], out_len[i]))
+    return result
+
+
 class Deflate:
     """`Deflate(bytes, level: 6, windowBits: 15)` (lib/src/codecs/zlib/deflate.dart:25-100): raw DEFLATE produced in the
     constructor, `get_bytes()` / `take_bytes()`, and `crc32` of the consumed input.  Invalid parameters make the

@@ -3470,8 +3470,62 @@ int b200z_crc64(const uint8_t *in, size_t in_len, uint64_t *crc) {
   CU(cudaSetDevice(g.device));
   return xz_crc64_impl(in, in_len, crc, g.stream);
 }
-// (debug, not part of the ABI) k_xz_lzma time in ms and the run count of the last b200z_xz_decode
+// (debug, not part of the ABI) k_xz_lzma time in ms and the run count of the last b200z_xz_decode*
 void b200z_debug_xz(double *lzma_ms, uint32_t *n_runs) { xz_debug(lzma_ms, n_runs); }
+
+// the argument rules of the XZ batch entries (those of the BZip2 ones): no null array, no range that wraps, no output
+// slots that overlap; nothing is written when one is broken
+static int xz_batch_args(const char *name, const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                         uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  if (n && (!in_off || !in_len || !out_off || !out_cap || !out_len || !rc)) {
+    set_err("%s: null array", name);
+    return B200Z_E_ARG;
+  }
+  std::vector<size_t> by_out;
+  for (size_t i = 0; i < n; ++i) {
+    if (in_off[i] + in_len[i] < in_off[i] || out_off[i] + out_cap[i] < out_off[i] || (in_len[i] && !in_base) ||
+        (out_cap[i] && !out_base)) {
+      set_err("%s: stream %zu: bad range", name, i);
+      return B200Z_E_ARG;
+    }
+    if (out_cap[i]) by_out.push_back(i);
+  }
+  std::sort(by_out.begin(), by_out.end(), [&](size_t a, size_t b) { return out_off[a] < out_off[b]; });
+  for (size_t k = 1; k < by_out.size(); ++k)
+    if (out_off[by_out[k - 1]] + out_cap[by_out[k - 1]] > out_off[by_out[k]]) {
+      set_err("%s: output slots %zu and %zu overlap", name, by_out[k - 1], by_out[k]);
+      return B200Z_E_ARG;
+    }
+  return B200Z_OK;
+}
+int b200z_xz_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  r = xz_batch_args("xz_decode_batch", in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, rc);
+  if (r) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return xz_decode_streams(in_base, in_off, in_len, n, verify, out_base, out_off, out_cap, out_len, rc, g.stream);
+}
+int b200z_xz_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
+                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  if (check < 0 || check > 3) {
+    set_err("xz_encode_batch: check must be 0 (none), 1 (crc32), 2 (crc64) or 3 (sha256)");
+    return B200Z_E_ARG;
+  }
+  r = xz_batch_args("xz_encode_batch", in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, rc);
+  if (r || n == 0) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return xz_encode_streams(in_base, in_off, in_len, n, check, out_base, out_off, out_cap, out_len, rc, g.stream);
+}
+// (test hooks, not part of the ABI) cap on the streams of one XZ decode device group (0: the memory budget alone); the
+// last b200z_xz_decode* call's streams, device groups and runs
+void b200z_debug_xz_batch_set(unsigned max_streams) { xz_batch_set(max_streams); }
+void b200z_debug_xz_batch_stats(unsigned long long out[3]) { xz_batch_stats(out); }
 
 int b200z_bzip2_decode_shard(const uint8_t *in, size_t in_len, uint32_t rank, uint32_t world, uint8_t *out, size_t out_cap,
                              size_t *out_len, b200z_bz2_block *blocks, size_t blocks_cap, size_t *n_blocks) {

@@ -217,10 +217,21 @@ cudaError_t zip_launch_zipcrypto(const ZipCryptoMember *d_m, uint32_t n, const u
 
 // ---- XZ (xz_kernels.cu): host buffers in, host buffers out, blocking on `s` ----
 size_t xz_bound(const uint8_t *in, size_t n);  // the output the container declares, up to where its walk stops
+// n streams (arguments checked): rc[i] / out_len[i] / bytes as xz_decode_impl / xz_encode_impl give for stream i alone;
+// the return value is B200Z_OK, B200Z_E_ARG (encode: a bad check kind) or a device failure
+int xz_decode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                      uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
+                      cudaStream_t s);
+int xz_encode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
+                      uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
+                      cudaStream_t s);
+// the batch of one
 int xz_decode_impl(const uint8_t *in, size_t n, int verify, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s);
 int xz_crc64_impl(const uint8_t *in, size_t n, uint64_t *crc, cudaStream_t s);
 size_t xz_encode_bound(size_t n);
 int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s);
-void xz_debug(double *lzma_ms, uint32_t *n_runs);  // k_xz_lzma time (CUDA events) and run count of the last decode
+void xz_debug(double *lzma_ms, uint32_t *n_runs);  // k_xz_lzma time (CUDA events) and run count of the last decode call
+void xz_batch_set(uint32_t max_streams);           // test hook: streams per device group (0: the memory budget alone)
+void xz_batch_stats(unsigned long long out[3]);    // the last decode call's streams, device groups and runs
 
 }  // namespace b200z

@@ -21,9 +21,11 @@
 //                 before its own first byte, because a reach before dictionary position 0 is an error of its own.
 //                 Per chunk: XZ_OK, or XZ_OVERSHOOT / XZ_READPAST / XZ_REACH / XZ_POSSTATE, each a Dart throw (see
 //                 DESIGN.md section 7 for the overshoot case).
-//   k_crc64_tiles CRC-64 of 64 KiB tiles (one thread each); the host folds them with x^(8n) mod P.  CRC-32 checks go
-//                 through the library's CRC-32 tile path (device_crc32_on).
-//   k_xz_sha256   one thread per message (the encoder's SHA-256 check).
+//   k_crc_tiles   CRC-64 (64 KiB tiles) or CRC-32 (8 KiB tiles) of a tile table, one thread each; the host folds them
+//                 with x^(8n) mod P.
+//   k_xz_sha256   one thread per message of a table (the encoder's SHA-256 check).
+//   batches       b200z_xz_decode_batch / _encode_batch: the plans of many streams in one table, each kernel launched
+//                 once per device group; the single calls are batches of one.
 //
 // Built by nvcc for sm_90a (product).  The CPU emulation build of the library compiles this file as part of b200z_api.cu,
 // which includes it under B200Z_EMU; the launches go through XZ_LAUNCH so that both compilers take them.
@@ -72,6 +74,7 @@ struct XzChunk {
 struct XzRun {
   uint32_t first, n;       // chunks [first, first + n)
   uint64_t bytes;          // output bytes (the ordering key)
+  uint64_t out0;           // its first output byte: nothing in front of it belongs to the run
   uint32_t global_slot;    // 0xffffffff: model in shared memory
   uint32_t lclp_max;
 };
@@ -323,8 +326,10 @@ __global__ void __launch_bounds__(32) k_xz_lzma(const uint8_t *__restrict__ in, 
         lz.s = XzState{0, 0, 0, 0, 0};
       }
       if (!c.lzma) continue;  // stored: k_xz_copy has written it
-      // the ring starts as the output in front of the chunk (earlier chunks of the run, stored ones included)
-      const uint64_t pre = min((uint64_t)XZ_WIN, c.out_off);
+      // the ring starts as the output in front of the chunk (earlier chunks of the run, stored ones included).  Bytes
+      // before the run's first byte are never read: they belong to another run, or another stream, which another CTA
+      // may be writing (XZ_REACH keeps every reach inside the run, so the ring never needs them).
+      const uint64_t pre = min((uint64_t)XZ_WIN, c.out_off - run.out0);
       for (uint32_t i = lane; i < pre; i += 32) {
         const uint64_t q = c.out_off - pre + i;
         sm_ring[q & (XZ_WIN - 1)] = out[q];
@@ -374,13 +379,18 @@ __global__ void __launch_bounds__(32) k_xz_lzma(const uint8_t *__restrict__ in, 
   }
 }
 
-__global__ void __launch_bounds__(256) k_crc64_tiles(const uint8_t *__restrict__ d, const uint64_t *__restrict__ tile_off,
-                                                     const uint32_t *__restrict__ tile_len, uint32_t n_tiles,
-                                                     uint64_t *__restrict__ part) {
-  __shared__ uint64_t tab[256];
+// CRC of each tile of a table (any offsets, any lengths), one thread each; W = uint64_t is CRC-64 (ECMA-182, the XZ
+// check and getCrc64), W = uint32_t its CRC-32 twin (the XZ CRC-32 check).  Both reflected, with all-ones in and out.
+constexpr uint64_t XZ_POLY64 = 0xC96C5795D7870F42ull;
+constexpr uint32_t XZ_POLY32 = 0xEDB88320u;
+template <class W>
+__global__ void __launch_bounds__(256) k_crc_tiles(const uint8_t *__restrict__ d, const uint64_t *__restrict__ tile_off,
+                                                   const uint32_t *__restrict__ tile_len, uint32_t n_tiles, W poly,
+                                                   W *__restrict__ part) {
+  __shared__ W tab[256];
   {
-    uint64_t c = threadIdx.x;
-    for (int k = 0; k < 8; ++k) c = (c & 1) ? 0xC96C5795D7870F42ull ^ (c >> 1) : c >> 1;
+    W c = threadIdx.x;
+    for (int k = 0; k < 8; ++k) c = (c & 1) ? poly ^ (c >> 1) : c >> 1;
     tab[threadIdx.x] = c;
   }
   __syncthreads();
@@ -388,8 +398,17 @@ __global__ void __launch_bounds__(256) k_crc64_tiles(const uint8_t *__restrict__
   if (t >= n_tiles) return;
   const uint8_t *p = d + tile_off[t];
   const uint32_t n = tile_len[t];
-  uint64_t c = ~0ull;
-  for (uint32_t i = 0; i < n; ++i) c = tab[(c ^ p[i]) & 0xff] ^ (c >> 8);
+  W c = ~(W)0;
+  uint32_t i = 0;
+  if (((uintptr_t)p & 15) == 0) {  // 16-byte words where the tile is aligned
+    for (; i + 16 <= n; i += 16) {
+      const uint4 v = *(const uint4 *)(p + i);
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+      for (int k = 0; k < 4; ++k)
+        for (int b = 0; b < 4; ++b) c = tab[(c ^ (w[k] >> (8 * b))) & 0xff] ^ (c >> 8);
+    }
+  }
+  for (; i < n; ++i) c = tab[(c ^ p[i]) & 0xff] ^ (c >> 8);
   part[t] = ~c;
 }
 
@@ -406,6 +425,7 @@ __device__ void xz_sha256_block(uint32_t h[8], const uint8_t *p) {
   uint32_t w[16];
   for (int i = 0; i < 16; ++i) w[i] = (uint32_t)p[4 * i] << 24 | (uint32_t)p[4 * i + 1] << 16 | (uint32_t)p[4 * i + 2] << 8 | p[4 * i + 3];
   uint32_t a = h[0], b = h[1], c = h[2], d = h[3], e = h[4], f = h[5], g = h[6], hh = h[7];
+#pragma unroll  // constant indices keep the message schedule w[] in registers
   for (int i = 0; i < 64; ++i) {
     uint32_t wi;
     if (i < 16) {
@@ -421,8 +441,21 @@ __device__ void xz_sha256_block(uint32_t h[8], const uint8_t *p) {
   }
   h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
 }
-__global__ void __launch_bounds__(32) k_xz_sha256(const uint8_t *__restrict__ d, uint64_t n, uint8_t *__restrict__ digest) {
-  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+// one message of k_xz_sha256: bytes d[off, off + len), digest to digest[32 * slot, + 32)
+struct XzMsg {
+  uint64_t off, len;
+  uint32_t slot, pad_;
+};
+// one thread per message (SHA-256 is a serial chain); the table is sorted longest first, so the threads of a warp get
+// messages of similar lengths
+__global__ void __launch_bounds__(32) k_xz_sha256(const uint8_t *__restrict__ d, const XzMsg *__restrict__ msg, uint32_t n_msg,
+                                                  uint8_t *__restrict__ digest_base) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_msg) return;
+  const XzMsg m = msg[t];
+  const uint64_t n = m.len;
+  uint8_t *digest = digest_base + 32 * (size_t)m.slot;
+  d += m.off;
   uint32_t h[8] = {0x6a09e667, 0xbb67ae85, 0x3c6ef372, 0xa54ff53a, 0x510e527f, 0x9b05688c, 0x1f83d9ab, 0x5be0cd19};
   uint64_t i = 0;
   for (; i + 64 <= n; i += 64) xz_sha256_block(h, d + i);
@@ -438,29 +471,31 @@ __global__ void __launch_bounds__(32) k_xz_sha256(const uint8_t *__restrict__ d,
   for (int k = 0; k < 32; ++k) digest[k] = (uint8_t)(h[k / 4] >> (24 - 8 * (k % 4)));
 }
 
-// ---- host: CRC folding (x^(8n) mod P, as zlib's crc32_combine) ----
-static uint64_t crc64_mulmod(uint64_t a, uint64_t b) {
-  uint64_t m = 1ull << 63, p = 0;
+// ---- host: CRC folding (x^(8n) mod P, as zlib's crc32_combine), for CRC-64 and CRC-32 alike ----
+// a * b mod P in the reflected representation (the top bit is x^0)
+template <class W>
+static W xz_mulmod(W a, W b, W poly) {
+  W m = (W)1 << (8 * sizeof(W) - 1), p = 0;
   for (;;) {
     if (a & m) {
       p ^= b;
       if ((a & (m - 1)) == 0) break;
     }
     m >>= 1;
-    b = (b & 1) ? (b >> 1) ^ 0xC96C5795D7870F42ull : b >> 1;
+    b = (b & 1) ? (b >> 1) ^ poly : b >> 1;
   }
   return p;
 }
-// CRC-64 of A || B from crc(A), crc(B) and |B| (crc(A) * x^(8|B|) + crc(B), as zlib's crc32_combine does for CRC-32)
-static uint64_t crc64_combine(uint64_t ca, uint64_t cb, uint64_t len_b) {
-  uint64_t x = 1ull << 55;  // x^8 (bit 63 = x^0)
-  uint64_t p = 1ull << 63;
-  while (len_b) {
-    if (len_b & 1) p = crc64_mulmod(x, p);
-    len_b >>= 1;
-    if (len_b) x = crc64_mulmod(x, x);
+template <class W>
+static W xz_xpow8(uint64_t n, W poly) {  // x^(8n) mod P
+  W x = (W)1 << (8 * sizeof(W) - 9);    // x^8
+  W p = (W)1 << (8 * sizeof(W) - 1);    // x^0
+  while (n) {
+    if (n & 1) p = xz_mulmod(x, p, poly);
+    n >>= 1;
+    if (n) x = xz_mulmod(x, x, poly);
   }
-  return crc64_mulmod(p, ca) ^ cb;
+  return p;
 }
 
 // ---- host: the container walk (xz_decoder.dart:46-458 without the LZMA decode) ----
@@ -795,6 +830,8 @@ XzBuf x_in, x_out, x_meta, x_models;
 cudaEvent_t x_ev[2] = {nullptr, nullptr};
 double g_xz_lzma_ms = 0;
 uint32_t g_xz_runs = 0;
+uint32_t g_xz_max_group = 0;                    // test hook: streams per device group (0: the memory budget alone)
+unsigned long long g_xz_stats[3] = {0, 0, 0};  // the last decode call's streams, device groups and runs
 }  // namespace
 
 #define XZ_CU(x)                                                                               \
@@ -810,52 +847,129 @@ uint32_t g_xz_runs = 0;
 
 static inline size_t xz_align(size_t v) { return (v + 255) & ~(size_t)255; }
 
-// CRC-64 (c64) or CRC-32 of each [lo, hi) range of device bytes d.  CRC-32 is the library's tile path (device_crc32_on,
-// b200z_api.cu); CRC-64 is k_crc64_tiles over 64 KiB tiles of all ranges in one launch, folded here.
-static int xz_device_crcs(const uint8_t *d, const std::vector<std::pair<uint64_t, uint64_t>> &ranges, bool c64,
-                          std::vector<uint64_t> *crcs, cudaStream_t s) {
-  crcs->clear();
-  if (!c64) {
-    for (auto &r : ranges) {
-      XZ_CU(x_meta.reserve(((r.second - r.first) / 8192 + 1) * 4 + 256));
-      uint32_t c = 0;
-      const int rc = device_crc32_on(d + r.first, (size_t)(r.second - r.first), (uint32_t *)x_meta.p, s, &c);
-      if (rc) return rc;
-      crcs->push_back(c);
-    }
-    return B200Z_OK;
+namespace {
+// the host image of a device metadata area (x_meta): every table goes up in one copy; the results lie at its end and
+// come back in one copy
+struct XzMeta {
+  std::vector<uint8_t> h;
+  template <class T>
+  size_t put(const T *p, size_t count) {
+    const size_t o = xz_align(h.size());
+    h.resize(o + count * sizeof(T));
+    if (count) memcpy(h.data() + o, p, count * sizeof(T));
+    return o;
   }
-  const uint64_t TILE = 1u << 16;
-  std::vector<uint64_t> toff;
-  std::vector<uint32_t> tlen;
-  for (auto &r : ranges)
-    for (uint64_t o = r.first; o < r.second; o += TILE) {
-      toff.push_back(o);
-      tlen.push_back((uint32_t)std::min(TILE, r.second - o));
+  size_t zeros(size_t bytes) {
+    const size_t o = xz_align(h.size());
+    h.resize(o + bytes);
+    return o;
+  }
+};
+
+// CRC-64 or CRC-32 of many [lo, hi) ranges of device bytes: their tiles (64 KiB for CRC-64, 8 KiB for CRC-32) in one
+// k_crc_tiles launch, folded per range on the host
+struct XzTiles {
+  bool c64;
+  uint64_t tile, full;  // tile bytes; x^(8 tile) mod P
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> len;
+  std::vector<size_t> first{0};  // range r is tiles [first[r], first[r + 1])
+  size_t o_off = 0, o_len = 0, o_part = 0;  // where the table and the tile CRCs lie in the metadata area
+  explicit XzTiles(bool c)
+      : c64(c), tile(c ? 1u << 16 : 1u << 13),
+        full(c ? xz_xpow8<uint64_t>(1u << 16, XZ_POLY64) : xz_xpow8<uint32_t>(1u << 13, XZ_POLY32)) {}
+  size_t ranges() const { return first.size() - 1; }
+  void add(uint64_t lo, uint64_t hi) {
+    for (uint64_t o = lo; o < hi; o += tile) {
+      off.push_back(o);
+      len.push_back((uint32_t)std::min(tile, hi - o));
     }
-  const size_t nt = toff.size();
-  std::vector<uint64_t> part(nt);
-  if (nt) {
-    const size_t b_off = 0, b_len = xz_align(8 * nt), b_part = b_len + xz_align(4 * nt);
-    XZ_CU(x_meta.reserve(b_part + 8 * nt));
-    uint8_t *m = (uint8_t *)x_meta.p;
-    XZ_CU(cudaMemcpyAsync(m + b_off, toff.data(), 8 * nt, cudaMemcpyHostToDevice, s));
-    XZ_CU(cudaMemcpyAsync(m + b_len, tlen.data(), 4 * nt, cudaMemcpyHostToDevice, s));
-    XZ_LAUNCH(k_crc64_tiles, (unsigned)((nt + 255) / 256), 256, s, d, (const uint64_t *)(m + b_off),
-              (const uint32_t *)(m + b_len), (uint32_t)nt, (uint64_t *)(m + b_part));
+    first.push_back(off.size());
+  }
+  void put_table(XzMeta &m) {
+    o_off = m.put(off.data(), off.size());
+    o_len = m.put(len.data(), len.size());
+  }
+  void put_result(XzMeta &m) { o_part = m.zeros(off.size() * (c64 ? 8 : 4)); }
+  void launch(const uint8_t *d, uint8_t *m, cudaStream_t s) const {
+    const uint32_t nt = (uint32_t)off.size();
+    if (!nt) return;
+    const unsigned grid = (nt + 255) / 256;
+    if (c64)
+      XZ_LAUNCH(k_crc_tiles<uint64_t>, grid, 256, s, d, (const uint64_t *)(m + o_off), (const uint32_t *)(m + o_len), nt,
+                XZ_POLY64, (uint64_t *)(m + o_part));
+    else
+      XZ_LAUNCH(k_crc_tiles<uint32_t>, grid, 256, s, d, (const uint64_t *)(m + o_off), (const uint32_t *)(m + o_len), nt,
+                XZ_POLY32, (uint32_t *)(m + o_part));
     count_launch();
-    XZ_CU(cudaGetLastError());
-    XZ_CU(cudaMemcpyAsync(part.data(), m + b_part, 8 * nt, cudaMemcpyDeviceToHost, s));
-    XZ_CU(cudaStreamSynchronize(s));
   }
-  size_t t = 0;
-  for (auto &r : ranges) {
-    uint64_t c = 0;  // the CRC of nothing
-    for (uint64_t o = r.first; o < r.second; o += TILE, ++t) c = crc64_combine(c, part[t], tlen[t]);
-    crcs->push_back(c);
+  // the CRC of range r; `res` is the host copy of the metadata area from byte `res0` on
+  uint64_t crc(size_t r, const uint8_t *res, size_t res0) const {
+    if (c64) return fold<uint64_t>(r, (const uint64_t *)(res + (o_part - res0)), XZ_POLY64);
+    return fold<uint32_t>(r, (const uint32_t *)(res + (o_part - res0)), XZ_POLY32);
   }
+  template <class W>
+  W fold(size_t r, const W *part, W poly) const {
+    W c = 0;  // the CRC of nothing
+    for (size_t t = first[r]; t < first[r + 1]; ++t)
+      c = xz_mulmod<W>(len[t] == tile ? (W)full : xz_xpow8<W>(len[t], poly), c, poly) ^ part[t];
+    return c;
+  }
+};
+
+// one copy of the inputs of streams idx[0..m) to x_in: the span of them as it is, or the inputs packed (16-byte aligned)
+// when the span is mostly other bytes.  in_dev[j]: where stream idx[j] starts in x_in.
+int xz_stage(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, const size_t *idx, size_t m,
+             std::vector<uint64_t> *in_dev, cudaStream_t s) {
+  in_dev->assign(m, 0);
+  uint64_t lo = ~0ull, hi = 0, total = 0;
+  for (size_t j = 0; j < m; ++j) {
+    const size_t i = idx[j];
+    if (!in_len[i]) continue;
+    lo = std::min(lo, in_off[i]);
+    hi = std::max(hi, in_off[i] + in_len[i]);
+    total += (in_len[i] + 15) & ~15ull;
+  }
+  if (total == 0) return B200Z_OK;
+  std::vector<uint8_t> packed;
+  const uint8_t *src = in_base + lo;
+  size_t staged = (size_t)(hi - lo);
+  if (hi - lo <= 2 * total + ((uint64_t)1 << 20)) {
+    for (size_t j = 0; j < m; ++j) (*in_dev)[j] = in_len[idx[j]] ? in_off[idx[j]] - lo : 0;
+  } else {
+    packed.resize(total);
+    staged = 0;
+    for (size_t j = 0; j < m; ++j) {
+      const size_t i = idx[j];
+      (*in_dev)[j] = staged;
+      if (in_len[i]) memcpy(packed.data() + staged, in_base + in_off[i], in_len[i]);
+      staged += (in_len[i] + 15) & ~15ull;
+    }
+    src = packed.data();
+  }
+  XZ_CU(x_in.reserve(staged + 16));
+  XZ_CU(cudaMemcpyAsync(x_in.p, src, staged, cudaMemcpyHostToDevice, s));
   return B200Z_OK;
 }
+
+// half of what the device has free (with this file's buffers counted as free), at least 1 GiB, at most 24 GiB
+int xz_budget(uint64_t *budget) {
+  size_t free_b = 0, total_b = 0;
+  XZ_CU(cudaMemGetInfo(&free_b, &total_b));
+  const uint64_t avail = (uint64_t)free_b + x_in.cap + x_out.cap + x_meta.cap + x_models.cap;
+  *budget = std::min<uint64_t>(std::max<uint64_t>(avail / 2, (uint64_t)1 << 30), (uint64_t)24 << 30);
+  return B200Z_OK;
+}
+
+// one stream of a decode batch
+struct XzJob {
+  size_t i;  // its index in the call
+  XzPlan p;
+  uint64_t out_dev = 0;                // its output in x_out
+  size_t chunk0 = 0, r32 = 0, r64 = 0;  // its first chunk and first CRC-32 / CRC-64 range in its group's tables
+  uint32_t n_global = 0, lclp = 0;     // its runs whose model needs a global slot, and their largest lc + lp
+};
+}  // namespace
 
 size_t xz_bound(const uint8_t *in, size_t n) {
   XzPlan p;
@@ -863,167 +977,281 @@ size_t xz_bound(const uint8_t *in, size_t n) {
   return (size_t)p.out_bytes;
 }
 
-int xz_decode_impl(const uint8_t *in, size_t n, int verify, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s) {
-  XzPlan p;
-  xz_plan(in, n, verify, &p);
-  if (p.out_bytes > out_cap) {
-    *out_len = (size_t)p.out_bytes;
-    set_error_text("xz_decode: out_cap is smaller than the output the stream declares (b200z_xz_bound)");
-    return B200Z_E_NOSPC;
+// Decode the planned streams jobs[0..m) as one device group: one copy up of the inputs and one of the tables, one
+// k_xz_copy, one k_xz_lzma over the runs of all streams, one CRC launch per check kind, one copy back of the chunk
+// statuses and tile CRCs.  Then each stream replays its own events, and its bytes go to its slot.
+static int xz_decode_group(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, XzJob *jobs, size_t m,
+                           uint8_t *out_base, const uint64_t *out_off, uint64_t *out_len, int32_t *rc, cudaStream_t s) {
+  // ---- the group's tables: chunks, runs and check ranges rebased onto the staged input and the device output ----
+  std::vector<size_t> idx(m);
+  std::vector<uint64_t> in_dev;
+  uint64_t out_total = 0;
+  size_t nc = 0;
+  for (size_t j = 0; j < m; ++j) {
+    idx[j] = jobs[j].i;
+    jobs[j].out_dev = out_total;
+    out_total += xz_align(jobs[j].p.out_bytes);
+    nc += jobs[j].p.chunks.size();
   }
-  const size_t nc = p.chunks.size(), nr = p.runs.size();
-  std::vector<int32_t> status(nc, XZ_OK);
-  XZ_CU(x_out.reserve(p.out_bytes + 16));
+  XZ_CU(x_out.reserve(out_total + 16));
   if (nc) {
-    XZ_CU(x_in.reserve(n + 16));
-    XZ_CU(cudaMemcpyAsync(x_in.p, in, n, cudaMemcpyHostToDevice, s));
-    // runs longest first; models that do not fit shared memory get a global slot
-    std::vector<uint32_t> order(nr);
-    for (size_t i = 0; i < nr; ++i) order[i] = (uint32_t)i;
-    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return p.runs[a].bytes > p.runs[b].bytes; });
-    std::vector<XzRun> runs(nr);
-    uint32_t n_global = 0, big_lclp = 0;
-    for (size_t i = 0; i < nr; ++i) {
-      runs[i] = p.runs[order[i]];
-      runs[i].global_slot = 0xffffffffu;
-      if (runs[i].lclp_max > XZ_SMEM_LCLP) {
-        big_lclp = std::max(big_lclp, runs[i].lclp_max);
-        runs[i].global_slot = n_global++;
-      }
+    const int r = xz_stage(in_base, in_off, in_len, idx.data(), m, &in_dev, s);
+    if (r) return r;
+  }
+  std::vector<XzChunk> ch;
+  std::vector<XzRun> runs;
+  std::vector<uint32_t> stored;
+  XzTiles t32(false), t64(true);
+  ch.reserve(nc);
+  for (size_t j = 0; j < m; ++j) {
+    XzJob &J = jobs[j];
+    const XzPlan &p = J.p;
+    J.chunk0 = ch.size();
+    J.r32 = t32.ranges();
+    J.r64 = t64.ranges();
+    const uint32_t run0 = (uint32_t)runs.size();
+    for (XzChunk c : p.chunks) {
+      c.in_off += in_dev[j];
+      c.out_off += J.out_dev;
+      c.run += run0;
+      if (!c.lzma && c.in_len) stored.push_back((uint32_t)ch.size());
+      ch.push_back(c);
     }
-    for (auto &r : runs)
-      if (r.global_slot != 0xffffffffu) r.lclp_max = big_lclp;  // one slot size for all of them
-    std::vector<uint32_t> stored;
-    for (size_t i = 0; i < nc; ++i)
-      if (!p.chunks[i].lzma && p.chunks[i].in_len) stored.push_back((uint32_t)i);
-    const size_t o_ch = 0, o_runs = xz_align(nc * sizeof(XzChunk)), o_st = o_runs + xz_align(nr * sizeof(XzRun)),
-                 o_list = o_st + xz_align(4 * nc), o_ctr = o_list + xz_align(4 * stored.size() + 4), total = o_ctr + 256;
-    XZ_CU(x_meta.reserve(total));
-    uint8_t *m = (uint8_t *)x_meta.p;
-    XZ_CU(cudaMemcpyAsync(m + o_ch, p.chunks.data(), nc * sizeof(XzChunk), cudaMemcpyHostToDevice, s));
-    XZ_CU(cudaMemcpyAsync(m + o_runs, runs.data(), nr * sizeof(XzRun), cudaMemcpyHostToDevice, s));
-    if (!stored.empty()) XZ_CU(cudaMemcpyAsync(m + o_list, stored.data(), 4 * stored.size(), cudaMemcpyHostToDevice, s));
-    XZ_CU(cudaMemsetAsync(m + o_st, 0, 4 * nc, s));
-    XZ_CU(cudaMemsetAsync(m + o_ctr, 0, 4, s));
-    if (n_global) XZ_CU(x_models.reserve((size_t)n_global * xz_model_words(big_lclp) * 2));
-    const uint8_t *d_in = (const uint8_t *)x_in.p;
-    const XzChunk *d_ch = (const XzChunk *)(m + o_ch);
-    if (!stored.empty()) {
-      XZ_LAUNCH(k_xz_copy, (unsigned)stored.size(), 256, s, d_in, d_ch, (const uint32_t *)(m + o_list), (uint8_t *)x_out.p);
-      count_launch();
+    for (XzRun r : p.runs) {
+      r.out0 = J.out_dev + p.chunks[r.first].out_off;
+      r.first += (uint32_t)J.chunk0;
+      runs.push_back(r);
     }
+    for (const XzCheck &c : p.checks) (c.c64 ? t64 : t32).add(J.out_dev + c.lo, J.out_dev + c.hi);
+  }
+  // runs longest first across the group; models that do not fit shared memory get a global slot, all of one size
+  const size_t nr = runs.size();
+  std::vector<uint32_t> order(nr);
+  for (size_t i = 0; i < nr; ++i) order[i] = (uint32_t)i;
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return runs[a].bytes > runs[b].bytes; });
+  std::vector<XzRun> sorted(nr);
+  uint32_t n_global = 0, big_lclp = 0;
+  for (size_t i = 0; i < nr; ++i) {
+    sorted[i] = runs[order[i]];
+    sorted[i].global_slot = 0xffffffffu;
+    if (sorted[i].lclp_max > XZ_SMEM_LCLP) {
+      big_lclp = std::max(big_lclp, sorted[i].lclp_max);
+      sorted[i].global_slot = n_global++;
+    }
+  }
+  for (auto &r : sorted)
+    if (r.global_slot != 0xffffffffu) r.lclp_max = big_lclp;
+  XzMeta M;
+  const size_t o_ch = M.put(ch.data(), nc), o_runs = M.put(sorted.data(), nr), o_list = M.put(stored.data(), stored.size());
+  t32.put_table(M);
+  t64.put_table(M);
+  const size_t o_ctr = M.zeros(4), o_st = M.zeros(4 * nc);  // results from o_st on
+  t32.put_result(M);
+  t64.put_result(M);
+  const size_t o_end = M.h.size();
+  XZ_CU(x_meta.reserve(o_end));
+  if (n_global) XZ_CU(x_models.reserve((size_t)n_global * xz_model_words(big_lclp) * 2));
+  uint8_t *m_d = (uint8_t *)x_meta.p;
+  XZ_CU(cudaMemcpyAsync(m_d, M.h.data(), o_end, cudaMemcpyHostToDevice, s));
+  // ---- launches ----
+  const uint8_t *d_in = (const uint8_t *)x_in.p;
+  const XzChunk *d_ch = (const XzChunk *)(m_d + o_ch);
+  if (!stored.empty()) {
+    XZ_LAUNCH(k_xz_copy, (unsigned)stored.size(), 256, s, d_in, d_ch, (const uint32_t *)(m_d + o_list), (uint8_t *)x_out.p);
+    count_launch();
+  }
+  if (nr) {
     if (!x_ev[0]) {  // created once, kept for the life of the library
       XZ_CU(cudaEventCreate(&x_ev[0]));
       XZ_CU(cudaEventCreate(&x_ev[1]));
     }
-    cudaEvent_t e0 = x_ev[0], e1 = x_ev[1];
-    XZ_CU(cudaEventRecord(e0, s));
+    XZ_CU(cudaEventRecord(x_ev[0], s));
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const unsigned grid = (unsigned)std::min<size_t>(nr, (size_t)sms * 6);  // 6 resident one-warp CTAs per SM (35 KB smem)
-    XZ_LAUNCH(k_xz_lzma, grid, 32, s, d_in, d_ch, (const XzRun *)(m + o_runs), (uint32_t)nr, (uint32_t *)(m + o_ctr),
-              (uint16_t *)x_models.p, (uint8_t *)x_out.p, (int32_t *)(m + o_st));
+    XZ_LAUNCH(k_xz_lzma, grid, 32, s, d_in, d_ch, (const XzRun *)(m_d + o_runs), (uint32_t)nr, (uint32_t *)(m_d + o_ctr),
+              (uint16_t *)x_models.p, (uint8_t *)x_out.p, (int32_t *)(m_d + o_st));
     count_launch();
     XZ_CU(cudaGetLastError());
-    XZ_CU(cudaEventRecord(e1, s));
-    XZ_CU(cudaMemcpyAsync(status.data(), m + o_st, 4 * nc, cudaMemcpyDeviceToHost, s));
-    XZ_CU(cudaStreamSynchronize(s));
+    XZ_CU(cudaEventRecord(x_ev[1], s));
+  }
+  // the checks: one CRC pass per kind over every verified block of every stream
+  t32.launch((const uint8_t *)x_out.p, m_d, s);
+  t64.launch((const uint8_t *)x_out.p, m_d, s);
+  XZ_CU(cudaGetLastError());
+  std::vector<uint8_t> res(o_end - o_st);
+  if (!res.empty()) XZ_CU(cudaMemcpyAsync(res.data(), m_d + o_st, res.size(), cudaMemcpyDeviceToHost, s));
+  XZ_CU(cudaStreamSynchronize(s));
+  if (nr) {
     float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    g_xz_lzma_ms = ms;
-    g_xz_runs = (uint32_t)nr;
+    cudaEventElapsedTime(&ms, x_ev[0], x_ev[1]);
+    g_xz_lzma_ms += ms;
   }
-  // the checks: one CRC pass over every verified block
-  std::vector<uint64_t> crc32s, crc64s;
-  {
-    std::vector<std::pair<uint64_t, uint64_t>> r32, r64;
-    for (auto &c : p.checks) (c.c64 ? r64 : r32).push_back({c.lo, c.hi});
-    int rc = xz_device_crcs((const uint8_t *)x_out.p, r32, false, &crc32s, s);
-    if (rc) return rc;
-    rc = xz_device_crcs((const uint8_t *)x_out.p, r64, true, &crc64s, s);
-    if (rc) return rc;
-  }
-  // replay the reference's order: the first chunk that throws, or the first failed check, ends the stream
-  int rc = p.status;
-  uint64_t got = p.out_bytes;
-  size_t i32 = 0, i64 = 0;
-  for (const XzEvent &e : p.events) {
-    if (!e.check) {
-      if (status[e.idx] != XZ_OK) {
-        static const char *why[] = {"", "a match runs past the chunk's declared size", "a read past the chunk's compressed bytes",
-                                    "a reach before dictionary position 0", "posState >= 12 (pb = 4 or 5)"};
-        char msg[160];
-        snprintf(msg, sizeof msg, "xz_decode: chunk %u: %s (Dart: RangeError)", e.idx, why[status[e.idx] & 7]);
-        set_error_text(msg);
-        rc = B200Z_E_THROW;
-        got = p.chunks[e.idx].out_off;
-        break;
-      }
-    } else {
-      const XzCheck &c = p.checks[e.idx];
-      const uint64_t have = c.c64 ? crc64s[i64++] : crc32s[i32++];
-      if (have != (c.c64 ? c.want : (c.want & 0xffffffffu))) {
-        set_error_text("xz_decode: block check mismatch");
-        rc = B200Z_E_DATA;
-        got = c.hi;
-        break;
+  g_xz_runs += (uint32_t)nr;
+  g_xz_stats[2] += nr;
+  // ---- each stream replays the reference's order: the first chunk that throws, or the first failed check, ends it ----
+  const int32_t *status = (const int32_t *)res.data();
+  uint64_t got_all = 0;
+  bool failed = false;
+  for (size_t j = 0; j < m; ++j) {
+    const XzJob &J = jobs[j];
+    const XzPlan &p = J.p;
+    int r = p.status;
+    uint64_t got = p.out_bytes;
+    size_t i32 = J.r32, i64 = J.r64;
+    for (const XzEvent &e : p.events) {
+      if (!e.check) {
+        const int32_t st = status[J.chunk0 + e.idx];
+        if (st != XZ_OK) {
+          static const char *why[] = {"", "a match runs past the chunk's declared size", "a read past the chunk's compressed bytes",
+                                      "a reach before dictionary position 0", "posState >= 12 (pb = 4 or 5)"};
+          char msg[160];
+          snprintf(msg, sizeof msg, "xz_decode: chunk %u: %s (Dart: RangeError)", e.idx, why[st & 7]);
+          set_error_text(msg);
+          r = B200Z_E_THROW;
+          got = p.chunks[e.idx].out_off;
+          break;
+        }
+      } else {
+        const XzCheck &c = p.checks[e.idx];
+        const uint64_t have = c.c64 ? t64.crc(i64++, res.data(), o_st) : t32.crc(i32++, res.data(), o_st);
+        if (have != (c.c64 ? c.want : (c.want & 0xffffffffu))) {
+          set_error_text("xz_decode: block check mismatch");
+          r = B200Z_E_DATA;
+          got = c.hi;
+          break;
+        }
       }
     }
+    if (r == p.status && r == B200Z_E_DATA) set_error_text("xz_decode: the stream is not valid XZ (decodeStream returned false)");
+    if (r == p.status && r == B200Z_E_THROW) set_error_text("xz_decode: the container walk reads past the input (Dart: RangeError)");
+    if (got)
+      XZ_CU(cudaMemcpyAsync(out_base + out_off[J.i], (const uint8_t *)x_out.p + J.out_dev, (size_t)got, cudaMemcpyDeviceToHost, s));
+    rc[J.i] = r;
+    out_len[J.i] = got;
+    got_all += got;
+    failed |= r != B200Z_OK;
   }
-  if (rc == p.status && rc == B200Z_E_DATA) set_error_text("xz_decode: the stream is not valid XZ (decodeStream returned false)");
-  if (rc == p.status && rc == B200Z_E_THROW) set_error_text("xz_decode: the container walk reads past the input (Dart: RangeError)");
-  if (got) XZ_CU(cudaMemcpyAsync(out, x_out.p, (size_t)got, cudaMemcpyDeviceToHost, s));
   XZ_CU(cudaStreamSynchronize(s));
-  *out_len = (size_t)got;
   // a damaged stream can declare far more output than it yields (each 6-byte LZMA chunk header up to 2 MiB): the
   // reservation made for it is not kept for the life of the library
-  if (rc != B200Z_OK && x_out.cap > ((size_t)64 << 20) && got < x_out.cap / 4) x_out.release();
-  return rc;
+  if (failed && x_out.cap > ((size_t)64 << 20) && got_all < x_out.cap / 4) x_out.release();
+  return B200Z_OK;
+}
+
+int xz_decode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                      uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
+                      cudaStream_t s) {
+  g_xz_lzma_ms = 0;
+  g_xz_runs = 0;
+  g_xz_stats[0] = n;
+  g_xz_stats[1] = g_xz_stats[2] = 0;
+  // every stream's own walk, clamps, events and checks
+  std::vector<XzJob> jobs;
+  jobs.reserve(n);
+  for (size_t i = 0; i < n; ++i) {
+    out_len[i] = 0;
+    rc[i] = B200Z_OK;
+    XzJob J;
+    J.i = i;
+    xz_plan(in_len[i] ? in_base + in_off[i] : in_base, (size_t)in_len[i], verify, &J.p);
+    if (J.p.out_bytes > out_cap[i]) {
+      out_len[i] = J.p.out_bytes;
+      rc[i] = B200Z_E_NOSPC;
+      set_error_text("xz_decode: out_cap is smaller than the output the stream declares (b200z_xz_bound)");
+      continue;
+    }
+    for (const XzRun &r : J.p.runs)
+      if (r.lclp_max > XZ_SMEM_LCLP) {
+        J.n_global++;
+        J.lclp = std::max(J.lclp, r.lclp_max);
+      }
+    jobs.push_back(std::move(J));
+  }
+  if (jobs.empty()) return B200Z_OK;
+  uint64_t budget = ~0ull;
+  if (jobs.size() > 1) {
+    const int r = xz_budget(&budget);
+    if (r) return r;
+  }
+  // consecutive streams in device groups whose input, output, tables and model slots fit the budget; the first stream
+  // of a group always goes in, so a stream too large for any group is decoded on its own as the single call does
+  for (size_t k = 0; k < jobs.size();) {
+    uint64_t bytes = 0, n_global = 0;
+    uint32_t lclp = 0;
+    size_t e = k;
+    for (; e < jobs.size(); ++e) {
+      const XzPlan &p = jobs[e].p;
+      uint64_t b2 = bytes + xz_align(in_len[jobs[e].i]) + xz_align(p.out_bytes) + p.chunks.size() * (sizeof(XzChunk) + 8) +
+                    p.runs.size() * sizeof(XzRun);
+      for (const XzCheck &c : p.checks) b2 += ((c.hi - c.lo) / 8192 + 1) * 20;
+      const uint64_t g2 = n_global + jobs[e].n_global;
+      const uint32_t l2 = std::max(lclp, jobs[e].lclp);
+      const uint64_t need = b2 + (g2 ? g2 * xz_model_words(l2) * 2 : 0);
+      if (e > k && ((g_xz_max_group && e - k >= g_xz_max_group) || need > budget)) break;
+      bytes = b2;
+      n_global = g2;
+      lclp = l2;
+    }
+    g_xz_stats[1]++;
+    const int r = xz_decode_group(in_base, in_off, in_len, jobs.data() + k, e - k, out_base, out_off, out_len, rc, s);
+    if (r) return r;
+    k = e;
+  }
+  return B200Z_OK;
+}
+
+int xz_decode_impl(const uint8_t *in, size_t n, int verify, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s) {
+  const uint64_t off = 0, len = n, cap = out_cap;
+  uint64_t got = 0;
+  int32_t r1 = B200Z_OK;
+  const int rc = xz_decode_streams(in, &off, &len, 1, verify, out, &off, &cap, &got, &r1, s);
+  *out_len = (size_t)got;
+  return rc ? rc : r1;
+}
+
+// CRC tiles over device bytes d, blocking: the table up, one launch, the tile CRCs back into *res (the metadata area
+// from byte *res0 on)
+static int xz_tiles_run(XzTiles &t, const uint8_t *d, std::vector<uint8_t> *res, size_t *res0, cudaStream_t s) {
+  if (t.off.empty()) return B200Z_OK;
+  XzMeta M;
+  t.put_table(M);
+  t.put_result(M);
+  *res0 = t.o_part;
+  XZ_CU(x_meta.reserve(M.h.size()));
+  uint8_t *m_d = (uint8_t *)x_meta.p;
+  XZ_CU(cudaMemcpyAsync(m_d, M.h.data(), t.o_part, cudaMemcpyHostToDevice, s));
+  t.launch(d, m_d, s);
+  XZ_CU(cudaGetLastError());
+  res->resize(M.h.size() - t.o_part);
+  XZ_CU(cudaMemcpyAsync(res->data(), m_d + t.o_part, res->size(), cudaMemcpyDeviceToHost, s));
+  XZ_CU(cudaStreamSynchronize(s));
+  return B200Z_OK;
 }
 
 int xz_crc64_impl(const uint8_t *in, size_t n, uint64_t *crc, cudaStream_t s) {
   XZ_CU(x_in.reserve(n + 16));
   if (n) XZ_CU(cudaMemcpyAsync(x_in.p, in, n, cudaMemcpyHostToDevice, s));
-  std::vector<uint64_t> c;
-  int rc = xz_device_crcs((const uint8_t *)x_in.p, {{0, n}}, true, &c, s);
+  XzTiles t(true);
+  t.add(0, n);
+  std::vector<uint8_t> res;
+  size_t res0 = 0;
+  const int rc = xz_tiles_run(t, (const uint8_t *)x_in.p, &res, &res0, s);
   if (rc) return rc;
-  *crc = c[0];
+  *crc = t.crc(0, res.data(), res0);
   return B200Z_OK;
 }
 
 size_t xz_encode_bound(size_t n) { return n + 256; }
 
-// XZEncoder.encodeStream (xz_encoder.dart:30-62): header, ONE stored chunk (its 16-bit length field is cut for inputs
-// over 64 KiB, :181-182), the check computed on the device, index, footer
-int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s) {
-  static const int FL[4] = {0, 1, 4, 0xa};
-  if (check < 0 || check > 3) {
-    set_error_text("xz_encode: check must be 0 (none), 1 (crc32), 2 (crc64) or 3 (sha256)");
-    return B200Z_E_ARG;
-  }
-  const int flags = FL[check];
-  std::vector<uint8_t> tail;  // check + index + footer
-  uint8_t digest[32];
-  uint64_t c = 0;
-  if (n > 0 && flags) {
-    XZ_CU(x_in.reserve(n + 64));
-    XZ_CU(cudaMemcpyAsync(x_in.p, in, n, cudaMemcpyHostToDevice, s));
-    if (flags == 0xa) {
-      XZ_CU(x_meta.reserve(64));
-      XZ_LAUNCH(k_xz_sha256, 1, 32, s, (const uint8_t *)x_in.p, (uint64_t)n, (uint8_t *)x_meta.p);
-      count_launch();
-      XZ_CU(cudaGetLastError());
-      XZ_CU(cudaMemcpyAsync(digest, x_meta.p, 32, cudaMemcpyDeviceToHost, s));
-      XZ_CU(cudaStreamSynchronize(s));
-    } else {
-      std::vector<uint64_t> cs;
-      int rc = xz_device_crcs((const uint8_t *)x_in.p, {{0, n}}, flags == 4, &cs, s);
-      if (rc) return rc;
-      c = cs[0];
-    }
-  }
-  std::vector<uint8_t> head = {253, 55, 122, 88, 90, 0, 0, (uint8_t)flags};
+// XZEncoder.encodeStream (xz_encoder.dart:30-62) around the check field `chk` (4, 8 or 32 bytes by flags): header, ONE
+// stored chunk (its 16-bit length field is cut for inputs over 64 KiB, :181-182), check, index, footer.  The input's
+// bytes go between head and tail.
+static void xz_container(size_t n, int flags, const uint8_t *chk, std::vector<uint8_t> *head_p, std::vector<uint8_t> *tail_p) {
+  std::vector<uint8_t> &head = *head_p, &tail = *tail_p;
+  head = {253, 55, 122, 88, 90, 0, 0, (uint8_t)flags};
+  tail.clear();
   auto put32 = [](std::vector<uint8_t> &v, uint32_t x) {
     for (int i = 0; i < 4; ++i) v.push_back((uint8_t)(x >> (8 * i)));
   };
@@ -1034,7 +1262,7 @@ int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t 
     v.push_back((uint8_t)(x & 0x7f));
   };
   put32(head, host_crc32(head.data() + 6, 2));
-  size_t body = 0, pad = 0, unpadded = 0;
+  size_t pad = 0, unpadded = 0;
   if (n > 0) {
     const uint8_t bh[8] = {2, 0, 0x21, 1, 0x16, 0, 0, 0};
     head.insert(head.end(), bh, bh + 8);
@@ -1042,17 +1270,12 @@ int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t 
     head.push_back(1);
     head.push_back((uint8_t)(((n - 1) >> 8) & 0xff));
     head.push_back((uint8_t)((n - 1) & 0xff));
-    body = n;
     const size_t after = head.size() + n + 1;
     pad = (4 - after % 4) % 4;
     tail.push_back(0);  // end marker
     tail.insert(tail.end(), pad, 0);
-    if (flags == 1) put32(tail, (uint32_t)c);
-    if (flags == 4) {
-      put32(tail, (uint32_t)c);
-      put32(tail, (uint32_t)(c >> 32));
-    }
-    if (flags == 0xa) tail.insert(tail.end(), digest, digest + 32);
+    const size_t ck = flags == 1 ? 4 : flags == 4 ? 8 : flags == 0xa ? 32 : 0;
+    tail.insert(tail.end(), chk, chk + ck);
     unpadded = (head.size() - 12) + n + tail.size() - pad;
   }
   std::vector<uint8_t> idx = {0};
@@ -1072,21 +1295,110 @@ int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t 
   tail.insert(tail.end(), f.begin(), f.end());
   tail.push_back(89);
   tail.push_back(90);
-  const size_t total = head.size() + body + tail.size();
-  *out_len = total;
-  if (total > out_cap) {
-    set_error_text("xz_encode: out_cap too small (b200z_xz_encode_bound)");
-    return B200Z_E_NOSPC;
+}
+
+// n XZEncoder().encodeBytes(data, check:) calls.  The checks are the device's: the inputs of a device group go up in one
+// copy, then one k_crc_tiles launch (CRC-32 / CRC-64, folded per stream here) or one k_xz_sha256 launch over a table of
+// all messages; the containers are written on the host.
+int xz_encode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
+                      uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
+                      cudaStream_t s) {
+  static const int FL[4] = {0, 1, 4, 0xa};
+  if (check < 0 || check > 3) {
+    set_error_text("xz_encode: check must be 0 (none), 1 (crc32), 2 (crc64) or 3 (sha256)");
+    return B200Z_E_ARG;
   }
-  memcpy(out, head.data(), head.size());
-  if (body) memcpy(out + head.size(), in, body);
-  memcpy(out + head.size() + body, tail.data(), tail.size());
+  const int flags = FL[check];
+  const size_t ck = flags == 1 ? 4 : flags == 4 ? 8 : flags == 0xa ? 32 : 0;
+  std::vector<uint8_t> chk(n * ck), head, tail;
+  std::vector<size_t> dev;  // the streams whose check the device computes
+  for (size_t i = 0; i < n; ++i) {
+    xz_container((size_t)in_len[i], flags, chk.data(), &head, &tail);
+    out_len[i] = head.size() + in_len[i] + tail.size();
+    rc[i] = B200Z_OK;
+    if (out_len[i] > out_cap[i]) {
+      set_error_text("xz_encode: out_cap too small (b200z_xz_encode_bound)");
+      rc[i] = B200Z_E_NOSPC;
+    } else if (in_len[i] && flags) {
+      dev.push_back(i);
+    }
+  }
+  uint64_t budget = ~0ull;
+  if (dev.size() > 1) {
+    const int r = xz_budget(&budget);
+    if (r) return r;
+  }
+  for (size_t k = 0; k < dev.size();) {
+    size_t e = k;
+    for (uint64_t bytes = 0; e < dev.size(); ++e) {
+      const uint64_t b2 = bytes + xz_align(in_len[dev[e]]) + (in_len[dev[e]] / 8192 + 1) * 20 + 64;
+      if (e > k && b2 > budget) break;
+      bytes = b2;
+    }
+    const size_t m = e - k;
+    std::vector<uint64_t> in_dev;
+    int r = xz_stage(in_base, in_off, in_len, dev.data() + k, m, &in_dev, s);
+    if (r) return r;
+    const uint8_t *d_in = (const uint8_t *)x_in.p;
+    if (flags == 0xa) {
+      // SHA-256: one thread per message, longest first
+      std::vector<XzMsg> msg(m);
+      for (size_t j = 0; j < m; ++j) msg[j] = XzMsg{in_dev[j], in_len[dev[k + j]], (uint32_t)j, 0};
+      std::stable_sort(msg.begin(), msg.end(), [](const XzMsg &a, const XzMsg &b) { return a.len > b.len; });
+      XzMeta M;
+      const size_t o_msg = M.put(msg.data(), m), o_dig = M.zeros(32 * m);
+      XZ_CU(x_meta.reserve(M.h.size()));
+      uint8_t *m_d = (uint8_t *)x_meta.p;
+      XZ_CU(cudaMemcpyAsync(m_d, M.h.data(), o_dig, cudaMemcpyHostToDevice, s));
+      XZ_LAUNCH(k_xz_sha256, (unsigned)((m + 31) / 32), 32, s, d_in, (const XzMsg *)(m_d + o_msg), (uint32_t)m, m_d + o_dig);
+      count_launch();
+      XZ_CU(cudaGetLastError());
+      std::vector<uint8_t> dig(32 * m);
+      XZ_CU(cudaMemcpyAsync(dig.data(), m_d + o_dig, 32 * m, cudaMemcpyDeviceToHost, s));
+      XZ_CU(cudaStreamSynchronize(s));
+      for (size_t j = 0; j < m; ++j) memcpy(chk.data() + 32 * dev[k + j], dig.data() + 32 * j, 32);
+    } else {
+      XzTiles t(flags == 4);
+      for (size_t j = 0; j < m; ++j) t.add(in_dev[j], in_dev[j] + in_len[dev[k + j]]);
+      std::vector<uint8_t> res;
+      size_t res0 = 0;
+      r = xz_tiles_run(t, d_in, &res, &res0, s);
+      if (r) return r;
+      for (size_t j = 0; j < m; ++j) {
+        const uint64_t c = t.crc(j, res.data(), res0);
+        for (size_t b = 0; b < ck; ++b) chk[ck * dev[k + j] + b] = (uint8_t)(c >> (8 * b));
+      }
+    }
+    k = e;
+  }
+  for (size_t i = 0; i < n; ++i) {
+    if (rc[i] != B200Z_OK) continue;
+    xz_container((size_t)in_len[i], flags, chk.data() + ck * i, &head, &tail);
+    uint8_t *out = out_base + out_off[i];
+    memcpy(out, head.data(), head.size());
+    if (in_len[i]) memcpy(out + head.size(), in_base + in_off[i], (size_t)in_len[i]);
+    memcpy(out + head.size() + in_len[i], tail.data(), tail.size());
+  }
   return B200Z_OK;
+}
+
+int xz_encode_impl(const uint8_t *in, size_t n, int check, uint8_t *out, size_t out_cap, size_t *out_len, cudaStream_t s) {
+  const uint64_t off = 0, len = n, cap = out_cap;
+  uint64_t got = 0;
+  int32_t r1 = B200Z_OK;
+  const int rc = xz_encode_streams(in, &off, &len, 1, check, out, &off, &cap, &got, &r1, s);
+  if (rc) return rc;
+  *out_len = (size_t)got;
+  return r1;
 }
 
 void xz_debug(double *lzma_ms, uint32_t *n_runs) {
   *lzma_ms = g_xz_lzma_ms;
   *n_runs = g_xz_runs;
+}
+void xz_batch_set(uint32_t max_streams) { g_xz_max_group = max_streams; }
+void xz_batch_stats(unsigned long long out[3]) {
+  for (int k = 0; k < 3; ++k) out[k] = g_xz_stats[k];
 }
 
 }  // namespace b200z

@@ -265,6 +265,12 @@ class B200Z {
   late final _Bz2DecodeD xzEncode = _lib.lookupFunction<_Bz2DecodeC, _Bz2DecodeD>('b200z_xz_encode');
   late final _SizeOfD xzEncodeBound = _lib.lookupFunction<_SizeOfC, _SizeOfD>('b200z_xz_encode_bound');
   late final _Crc64D crc64 = _lib.lookupFunction<_Crc64C, _Crc64D>('b200z_crc64');
+  // XZ batches: (inBase, inOff, inLen, n, verify | check, outBase, outOff, outCap, outLen, rc) -- the shape of
+  // b200z_bzip2_decode_batch
+  late final _Bz2DecodeBatchD xzDecodeBatch =
+      _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_xz_decode_batch');
+  late final _Bz2DecodeBatchD xzEncodeBatch =
+      _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_xz_encode_batch');
   late final _DeflateBatchD deflateBatch = _lib.lookupFunction<_DeflateBatchC, _DeflateBatchD>('b200z_deflate_batch');
   late final _InflateBatchD inflateBatch = _lib.lookupFunction<_InflateBatchC, _InflateBatchD>('b200z_inflate_batch');
   late final _InflateBatchDeviceD inflateBatchDevice =

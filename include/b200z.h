@@ -184,6 +184,22 @@ size_t b200z_xz_bound(const uint8_t *in, size_t in_len);
 int b200z_xz_encode(const uint8_t *in, size_t in_len, int check, uint8_t *out, size_t out_cap, size_t *out_len);
 size_t b200z_xz_encode_bound(size_t in_len);
 int b200z_crc64(const uint8_t *in, size_t in_len, uint64_t *crc);
+/* b200z_xz_decode_batch = n independent XZDecoder().decodeBytes(data, verify:) calls in one.  Stream i reads
+ * in_base[in_off[i] .. +in_len[i]) and writes out_base[out_off[i] .. +out_cap[i]); rc[i], out_len[i] and the bytes in its
+ * slot are exactly what b200z_xz_decode gives for that stream alone (OK / E_DATA / E_THROW / E_NOSPC with out_len[i] =
+ * b200z_xz_bound, which is the room that always suffices).  Input ranges may overlap or repeat; n == 0 returns OK.  Returns
+ * OK unless an argument is wrong (null arrays, wrapping ranges, overlapping output slots: B200Z_E_ARG and nothing is
+ * written) or the device fails.  The runs of all streams share one k_xz_lzma launch, so many single-block streams (one
+ * warp each) fill the GPU where one call per stream keeps one warp busy; streams are cut into consecutive device groups
+ * that fit the device memory.
+ * b200z_xz_encode_batch = n independent XZEncoder().encodeBytes(data, check:) calls in one, one check kind for all (0..3
+ * as b200z_xz_encode, anything else is B200Z_E_ARG); rc[i] / out_len[i] / bytes as b200z_xz_encode for that stream alone
+ * (E_NOSPC: out_len[i] = the size needed, b200z_xz_encode_bound always suffices).  The checks of all streams are one
+ * launch: CRC tiles, or SHA-256 with one thread per message.  The same argument rules as b200z_xz_decode_batch.      */
+int b200z_xz_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc);
+int b200z_xz_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
+                          uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc);
 
 /* ---- ZIP container: ZipDecoder / ZipDirectory / ZipFileHeader / ZipFile ------------------------------------
  * b200z_zip_list   = ZipDirectory.read (zip_directory.dart:25-183) + ZipFileHeader.read (zip_file_header.dart:28-111)

@@ -193,7 +193,7 @@ __device__ __forceinline__ void fp_sts16(uint32_t a, uint32_t v) {
 // g_fp_prof[phase] -- where the WALL time of a unit goes, barrier waits included (the instruction counts of the ncu source
 // page do not show those).  Read and cleared by b200z_debug_fast_prof.
 #ifdef FP_PROF
-__device__ unsigned long long g_fp_prof[20];
+__device__ unsigned long long g_fp_prof[24];
 #define FP_TICK(k)                                                          \
   do {                                                                      \
     if (tid == 0) {                                                         \
@@ -685,9 +685,20 @@ FP_DEV void fp_lz77_run(uint8_t *smem, uint32_t tid, uint32_t nthr, uint32_t ole
 #endif
     bool has = false;  // a match of mine is ready and waits for the warp's next copy turn
     uint32_t rp = 0, rlen = 0, rdist = 0, rb = 0;
+#ifdef FP_PROF
+    // lane 0 of each warp: clocks probing (the looks before a turn) and in copy turns; turns, the sum and the maximum of
+    // the ready lengths per turn; every lane: looks and failed looks.  Added to g_fp_prof[17 ..] when the pass ends.
+    unsigned long long pr_probe = 0, pr_copy = 0, pr_turns = 0, pr_tsum = 0, pr_tmax = 0;
+    uint32_t pr_looks = 0, pr_fail = 0;
+    long long pr_t = clock64();
+#define FP_LOOK(ok) (++pr_looks, pr_fail += (ok) ? 0u : 1u)
+#else
+#define FP_LOOK(ok)
+#endif
     for (;;) {
-      // ---- look for a ready match (lanes that hold one wait for the warp's next copy turn: copying with a few lanes
-      // costs the warp as much as copying with all of them, so two looks are taken before every turn) ----
+      // ---- look for a ready match (lanes that hold one wait for the warp's next copy turn).  With FP_TRIES > 1 a warp
+      // takes up to FP_TRIES looks before a turn and stops early once 20 lanes hold one; with one look per turn (the
+      // default) there is nothing to stop, and the vote is not taken: it cost 4 % of bench.py config 2 ----
 #pragma unroll 1
       for (int tries = 0; tries < FP_TRIES; ++tries) {
         if (!has && w < nitems) {
@@ -729,6 +740,7 @@ FP_DEV void fp_lz77_run(uint8_t *smem, uint32_t tid, uint32_t nthr, uint32_t ole
             cand &= cand - 1u;
             uint32_t len1, dist1;
             const bool r0 = probe(b0, len0, dist0), r1 = probe(b1, len1, dist1);
+            FP_LOOK(r0 || r1);
             if (r0 || r1) {
               has = true;
               rb = r0 ? b0 : b1;
@@ -737,7 +749,9 @@ FP_DEV void fp_lz77_run(uint8_t *smem, uint32_t tid, uint32_t nthr, uint32_t ole
               rp = (w >> G) * 32u + rb;
             }
 #else
-            if (probe(b0, len0, dist0)) {
+            const bool r0 = probe(b0, len0, dist0);
+            FP_LOOK(r0);
+            if (r0) {
               has = true;
               rb = b0;
               rlen = len0;
@@ -747,9 +761,23 @@ FP_DEV void fp_lz77_run(uint8_t *smem, uint32_t tid, uint32_t nthr, uint32_t ole
 #endif
           }
         }
-        if (tries == 0 && __popc(__ballot_sync(FULL, has)) >= 20) break;
+        if (FP_TRIES > 1 && tries == 0 && __popc(__ballot_sync(FULL, has)) >= 20) break;
       }
       if (__ballot_sync(FULL, has || w < nitems) == 0u) break;
+#ifdef FP_PROF
+      {
+        const unsigned ready = __ballot_sync(FULL, has);
+        const uint32_t tsum = __reduce_add_sync(FULL, has ? rlen : 0u), tmax = __reduce_max_sync(FULL, has ? rlen : 0u);
+        const long long t = clock64();
+        pr_probe += (unsigned long long)(t - pr_t);
+        pr_t = t;
+        if (ready) {
+          ++pr_turns;
+          pr_tsum += tsum;
+          pr_tmax += tmax;
+        }
+      }
+#endif
       if (has) {
         __threadfence_block();  // the bytes behind the clear bits are visible
         // overlapping run (dist < len, dist < STEP): [p - dist, p + k) is final and periodic, so any multiple of dist that
@@ -782,7 +810,30 @@ FP_DEV void fp_lz77_run(uint8_t *smem, uint32_t tid, uint32_t nthr, uint32_t ole
         f &= ~(1u << rb);
         has = false;
       }
+#ifdef FP_PROF
+      __syncwarp();
+      {
+        const long long t = clock64();
+        pr_copy += (unsigned long long)(t - pr_t);
+        pr_t = t;
+      }
+#endif
     }
+#ifdef FP_PROF
+    {
+      const uint32_t looks = __reduce_add_sync(FULL, pr_looks), fails = __reduce_add_sync(FULL, pr_fail);
+      if ((tid & 31u) == 0u) {
+        atomicAdd(&g_fp_prof[17], pr_probe);
+        atomicAdd(&g_fp_prof[18], pr_copy);
+        atomicAdd(&g_fp_prof[19], pr_turns);
+        atomicAdd(&g_fp_prof[20], pr_tsum);
+        atomicAdd(&g_fp_prof[21], pr_tmax);
+        atomicAdd(&g_fp_prof[22], (unsigned long long)looks);
+        atomicAdd(&g_fp_prof[23], (unsigned long long)fails);
+      }
+    }
+#endif
+#undef FP_LOOK
 #undef FP_ITEM_BITS
 }
 

@@ -565,8 +565,8 @@ cudaError_t launch_inflate(const InflateBatch &b, cudaStream_t stream) {
 
 #ifdef FP_PROF
 // FP_PROF builds only (scripts/build_variant.sh prof -DFP_PROF): k_inflate_fast's clocks per phase, summed over CTAs; cleared by the read.
-extern "C" int b200z_debug_fast_prof(unsigned long long *out16 /* [20] */) {
-  unsigned long long z[20] = {0};
+extern "C" int b200z_debug_fast_prof(unsigned long long *out16 /* [24] */) {
+  unsigned long long z[24] = {0};
   if (cudaMemcpyFromSymbol(out16, b200z::fp::g_fp_prof, sizeof z) != cudaSuccess) return -1;
   return cudaMemcpyToSymbol(b200z::fp::g_fp_prof, z, sizeof z) == cudaSuccess ? 0 : -1;
 }

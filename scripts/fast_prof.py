@@ -1,5 +1,6 @@
 """Where a unit's WALL time goes inside k_inflate_fast: bench.py's config-2 batch through an FP_PROF build
-(scripts/build_variant.sh prof -DFP_PROF; B200Z_LIB=archive_b200/variants/libb200z_prof.so) -- thread 0's clocks per phase."""
+(scripts/build_variant.sh prof -DFP_PROF; B200Z_LIB=archive_b200/variants/libb200z_prof.so) -- thread 0's clocks per phase,
+and inside the LZ77 pass: each warp's clocks probing against copying, copy turns, ready bytes per turn, looks."""
 import ctypes as C
 import os
 import sys
@@ -44,7 +45,7 @@ def main():
     for _ in range(3):
         step()
     torch.cuda.synchronize()
-    buf = (C.c_ulonglong * 20)()
+    buf = (C.c_ulonglong * 24)()
     L.b200z_debug_fast_prof(buf)
     reps = 5
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -62,6 +63,12 @@ def main():
     print("  waited at the closing barrier, mean over the 8 warps (clocks per unit; share of the phase):")
     for j, (name, ph) in enumerate([("pass A", 4), ("pass A2", 5), ("false-start count + scan", 7), ("pass C", 8), ("LZ77", 10)]):
         print(f"  {name:28s} {buf[12 + j] / k / 8:9.0f}  {100.0 * buf[12 + j] / 8 / max(buf[ph], 1):5.1f} %")
+    probe, copy, turns, tsum, tmax, looks, fails = buf[17:24]
+    print("  LZ77 pass, lane 0 of each warp, mean over the 8 warps (clocks per unit; share of the pass's clocks):")
+    print(f"  {'probing':28s} {probe / k / 8:9.0f}  {100.0 * probe / max(probe + copy, 1):5.1f} %")
+    print(f"  {'copy turns':28s} {copy / k / 8:9.0f}  {100.0 * copy / max(probe + copy, 1):5.1f} %")
+    print(f"  copy turns per unit {turns / k:.0f}; ready bytes per turn: sum {tsum / max(turns, 1):.1f}, longest match "
+          f"{tmax / max(turns, 1):.1f}; looks per unit {looks / k:.0f}, failed {100.0 * fails / max(looks, 1):.1f} %")
 
 
 if __name__ == "__main__":

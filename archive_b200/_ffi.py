@@ -84,6 +84,14 @@ _SIGS = {
     "b200z_xz_encode": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "b200z_xz_encode_bound": (C.c_size_t, [C.c_size_t]),
     "b200z_crc64": (C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64)]),
+    "b200z_gzip_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_zlib_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_gzip_encode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_uint32, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200z_zlib_encode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_xz_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200z_xz_encode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_void_p,

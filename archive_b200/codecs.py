@@ -419,6 +419,93 @@ def xz_encode_batch(contents, check: int = XZCheck.crc64) -> list:
     return result
 
 
+
+def _framed_decode_batch(call, streams, first_room) -> list:
+    """One gzip / zlib decode batch over `streams` -> [(rc, bytes)]; only the streams that got E_NOSPC are decoded
+    again, in larger rooms (bzip2_decode_batch's rule)."""
+    L = _ffi.ensure_init()
+    n = len(streams)
+    if n == 0:
+        return []
+    in_buf, in_off, in_len = _pack(streams)
+    base = C.addressof(in_buf)
+    rooms = [max(first_room(L, base + in_off[i], in_len[i]), 1 << 12) for i in range(n)]
+    result = [None] * n
+    todo = list(range(n))
+    while todo:
+        m = len(todo)
+        a_in_off = (C.c_uint64 * m)(*[in_off[i] for i in todo])
+        a_in_len = (C.c_uint64 * m)(*[in_len[i] for i in todo])
+        out, out_off, cap = _slots([rooms[i] for i in todo])
+        out_len = (C.c_uint64 * m)()
+        rc = (C.c_int32 * m)()
+        _ffi.check(call(L, base, a_in_off, a_in_len, m, C.addressof(out), out_off, cap, out_len, rc))
+        again = []
+        for k, i in enumerate(todo):
+            if rc[k] == _ffi.E_NOSPC and rooms[i] < (1 << 40):
+                rooms[i] = max(rooms[i] * 2, out_len[k] + (out_len[k] >> 3))
+                again.append(i)
+                continue
+            if rc[k] not in (_ffi.OK, _ffi.E_DATA, _ffi.E_THROW):
+                _ffi.check(rc[k])
+            result[i] = (rc[k], C.string_at(C.addressof(out) + out_off[k], out_len[k]))
+        todo = again
+    return result
+
+
+def gzip_decode_batch(streams, verify: bool = False, raw: bool = False) -> list:
+    """GZipDecoder().decodeBytes(stream, verify:, raw:) for every stream of `streams` in one b200z_gzip_decode_batch call:
+    a list of (rc, bytes) in the same order.  rc is what b200z_gzip_decode gives for that stream alone: OK, E_DATA
+    (decodeStream returned false) or E_THROW (the reference throws a RangeError), with the bytes written before it.
+    Rooms start at b200z_gzip_bound (4n + 1024 when that is unknown)."""
+    flags = int(bool(verify)) | (2 if raw else 0)  # B200Z_GZIP_VERIFY | B200Z_GZIP_RAW
+    return _framed_decode_batch(lambda L, b, io, il, m, o, oo, cap, ol, rc: L.b200z_gzip_decode_batch(b, io, il, m, flags, o, oo, cap, ol, rc),
+                                streams, lambda L, a, n: L.b200z_gzip_bound(a, n) or 4 * n + 1024)
+
+
+def zlib_decode_batch(streams, verify: bool = False, raw: bool = False) -> list:
+    """ZLibDecoder().decodeBytes(stream, verify:, raw:) for every stream of `streams` in one b200z_zlib_decode_batch call:
+    a list of (rc, bytes) as gzip_decode_batch gives them, each what b200z_zlib_decode gives for that stream alone."""
+    return _framed_decode_batch(lambda L, b, io, il, m, o, oo, cap, ol, rc: L.b200z_zlib_decode_batch(b, io, il, m, int(verify), int(raw),
+                                                                                                     o, oo, cap, ol, rc),
+                                streams, lambda L, a, n: 4 * n + 1024)
+
+
+def _framed_encode_batch(call, contents) -> list:
+    L = _ffi.ensure_init()
+    n = len(contents)
+    if n == 0:
+        return []
+    in_buf, in_off, in_len = _pack(contents)
+    out, out_off, cap = _slots([L.b200z_deflate_bound(in_len[i]) + 18 for i in range(n)])
+    out_len = (C.c_uint64 * n)()
+    rc = (C.c_int32 * n)()
+    _ffi.check(call(L, C.addressof(in_buf), in_off, in_len, n, C.addressof(out), out_off, cap, out_len, rc))
+    result = []
+    for i in range(n):
+        _ffi.check(rc[i])
+        result.append(C.string_at(C.addressof(out) + out_off[i], out_len[i]))
+    return result
+
+
+def gzip_encode_batch(contents, level: int = 6, mtime: int | None = None) -> list:
+    """GZipEncoder().encodeBytes(data, level:) for every input of `contents` in one b200z_gzip_encode_batch call: the
+    list of gzip streams in the same order, each identical to what GZipEncoder gives for that input alone with the same
+    `mtime` (the wall clock when None, read once for the whole batch)."""
+    import time
+    mt = int(time.time()) if mtime is None else mtime
+    return _framed_encode_batch(lambda L, b, io, il, n, o, oo, cap, ol, rc: L.b200z_gzip_encode_batch(b, io, il, n, level, mt, o, oo,
+                                                                                                     cap, ol, rc), contents)
+
+
+def zlib_encode_batch(contents, level: int = 6, window_bits: int = 15, raw: bool = False) -> list:
+    """ZLibEncoder().encodeBytes(data, level:, windowBits:, raw:) for every input of `contents` in one
+    b200z_zlib_encode_batch call: the list of streams in the same order, each what ZLibEncoder gives for it alone."""
+    return _framed_encode_batch(lambda L, b, io, il, n, o, oo, cap, ol, rc: L.b200z_zlib_encode_batch(b, io, il, n, level, window_bits,
+                                                                                                     int(raw), o, oo, cap, ol, rc),
+                                contents)
+
+
 class Deflate:
     """`Deflate(bytes, level: 6, windowBits: 15)` (lib/src/codecs/zlib/deflate.dart:25-100): raw DEFLATE produced in the
     constructor, `get_bytes()` / `take_bytes()`, and `crc32` of the consumed input.  Invalid parameters make the

@@ -116,7 +116,7 @@ struct Ctx {
   static const int kCompStreams = 8;
   cudaStream_t s_comp[kCompStreams] = {};
   DevBuf d_in, d_out, d_ws, d_meta, d_small, d_bz, d_tok, d_crypt;
-  PinBuf h_meta;
+  PinBuf h_meta, h_stage;  // h_stage: the outputs of a gzip / zlib decode batch on their way to the caller's slots (GZ_STAGE)
 };
 static Ctx g;
 
@@ -141,16 +141,21 @@ static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; 
 
 // ---------------------------------------------------------------------------------------------
 // Adler-32 on the device (adler32.dart:29-52).  s1 = 1 + sum b_i ; s2 = n + sum (n - i) b_i  (mod 65521)
-// Each block reduces a 64 KiB tile to (sum, weighted sum); the host folds the per-tile pairs (a few
-// integers per 64 KiB -- framing arithmetic, not a pass over the data).
+// Each block reduces one tile of at most 64 KiB to (sum, weighted sum); a launch takes the tiles of many messages.  The
+// host folds each message's per-tile pairs (a few integers per 64 KiB -- framing arithmetic, not a pass over the data).
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t ADLER_TILE = 1u << 16;
-__global__ void __launch_bounds__(256) k_adler_tiles(const uint8_t *__restrict__ p, size_t n, uint64_t *__restrict__ part) {
-  const size_t base = (size_t)blockIdx.x * ADLER_TILE;
-  const uint32_t len = (uint32_t)min((size_t)ADLER_TILE, n - base);
+struct AdlerTile {
+  uint64_t off;  // first byte, from the launch's base pointer
+  uint32_t len, pad_;
+};
+__global__ void __launch_bounds__(256) k_adler_tiles(const uint8_t *__restrict__ base, const AdlerTile *__restrict__ tiles,
+                                                     uint64_t *__restrict__ part) {
+  const uint8_t *p = base + tiles[blockIdx.x].off;
+  const uint32_t len = tiles[blockIdx.x].len;
   uint64_t s = 0, ws = 0;  // ws = sum (len - i) * b_i  within the tile
   for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) {
-    uint32_t b = p[base + i];
+    uint32_t b = p[i];
     s += b;
     ws += (uint64_t)(len - i) * b;
   }
@@ -175,31 +180,44 @@ __global__ void __launch_bounds__(256) k_adler_tiles(const uint8_t *__restrict__
   }
 }
 
+// Adler-32 of the n device messages base[off[m], off[m] + len[m]) with one launch and one synchronise (blocking)
+static int device_adler32_many(const uint8_t *base, const uint64_t *off, const uint64_t *len, size_t n, uint32_t *out) {
+  const uint32_t MOD = 65521;
+  std::vector<AdlerTile> tiles;
+  for (size_t m = 0; m < n; ++m)
+    for (uint64_t t = 0; t < len[m]; t += ADLER_TILE)
+      tiles.push_back({off[m] + t, (uint32_t)std::min<uint64_t>(ADLER_TILE, len[m] - t), 0});
+  std::vector<uint64_t> part(tiles.size() * 2);
+  if (!tiles.empty()) {
+    const size_t nt = tiles.size(), tab = align_up(nt * 16, 256);
+    CU(g.d_small.reserve(tab + nt * 16));
+    CU(cudaMemcpyAsync(g.d_small.p, tiles.data(), nt * sizeof(AdlerTile), cudaMemcpyHostToDevice, g.stream));
+    uint64_t *d_part = (uint64_t *)((uint8_t *)g.d_small.p + tab);
+    k_adler_tiles<<<(unsigned)nt, 256, 0, g.stream>>>(base, (const AdlerTile *)g.d_small.p, d_part);
+    count_launch();
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(part.data(), d_part, nt * 16, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+  }
+  size_t t = 0;
+  for (size_t m = 0; m < n; ++m) {
+    uint64_t s1 = 1, s2 = 0;
+    for (uint64_t at = 0; at < len[m]; at += ADLER_TILE, ++t) {
+      const uint64_t tl = std::min<uint64_t>(ADLER_TILE, len[m] - at);
+      uint64_t ts = part[2 * t] % MOD, tw = part[2 * t + 1] % MOD;
+      // appending a tile: s2' = s2 + len * s1 + tw ; s1' = s1 + ts
+      s2 = (s2 + (tl % MOD) * s1 + tw) % MOD;
+      s1 = (s1 + ts) % MOD;
+    }
+    out[m] = (uint32_t)((s2 << 16) | s1);
+  }
+  return B200Z_OK;
+}
+
 // device buffer -> adler32 (blocking)
 static int device_adler32(const uint8_t *d, size_t n, uint32_t *out) {
-  const uint32_t MOD = 65521;
-  if (n == 0) {
-    *out = 1;
-    return B200Z_OK;
-  }
-  size_t tiles = (n + ADLER_TILE - 1) / ADLER_TILE;
-  CU(g.d_small.reserve(tiles * 16));
-  k_adler_tiles<<<(unsigned)tiles, 256, 0, g.stream>>>(d, n, (uint64_t *)g.d_small.p);
-  count_launch();
-  CU(cudaGetLastError());
-  std::vector<uint64_t> part(tiles * 2);
-  CU(cudaMemcpyAsync(part.data(), g.d_small.p, tiles * 16, cudaMemcpyDeviceToHost, g.stream));
-  CU(cudaStreamSynchronize(g.stream));
-  uint64_t s1 = 1, s2 = 0;
-  for (size_t t = 0; t < tiles; ++t) {
-    uint64_t len = (t + 1 == tiles) ? n - t * ADLER_TILE : ADLER_TILE;
-    uint64_t ts = part[2 * t] % MOD, tw = part[2 * t + 1] % MOD;
-    // appending a tile: s2' = s2 + len * s1 + tw ; s1' = s1 + ts
-    s2 = (s2 + (len % MOD) * s1 + tw) % MOD;
-    s1 = (s1 + ts) % MOD;
-  }
-  *out = (uint32_t)((s2 << 16) | s1);
-  return B200Z_OK;
+  const uint64_t off = 0, len = n;
+  return device_adler32_many(d, &off, &len, 1, out);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -207,7 +225,7 @@ static int device_adler32(const uint8_t *d, size_t n, uint32_t *out) {
 // ---------------------------------------------------------------------------------------------
 struct MetaLayout {
   size_t n;
-  size_t off_in_off, off_out_off, off_in_len, off_out_cap, off_out_len, off_status, off_in_used, bytes;
+  size_t off_in_off, off_out_off, off_in_len, off_out_cap, off_out_len, off_status, off_in_used, off_hist, bytes;
   explicit MetaLayout(size_t n_) : n(n_) {
     size_t o = 0;
     off_in_off = o;
@@ -224,6 +242,8 @@ struct MetaLayout {
     o += 4 * n;
     off_in_used = o;
     o += 4 * n;
+    off_hist = o;  // (per-unit history, when a batch has one: InflateWs::unit_hist)
+    o += 4 * n;
     bytes = align_up(o, 256);
   }
   size_t inputs_bytes() const { return off_out_len; }
@@ -232,10 +252,12 @@ struct MetaLayout {
 static size_t workspace_bytes(size_t n_units, size_t total_out_cap) { return inflate_ws_bytes(n_units, total_out_cap); }
 
 // Runs one batch whose compressed bytes are ALREADY in g.d_in (at offset 0 = in_base) and whose
-// output goes to g.d_out.  Meta arrays are host arrays; results are copied back into them.
+// output goes to g.d_out.  Meta arrays are host arrays; results are copied back into them.  `unit_hist`: each unit's own
+// history (InflateWs::unit_hist), or null.
 static int run_batch_on_staged(const uint64_t *in_off, const uint32_t *in_len, const uint64_t *out_off,
                                const uint32_t *out_cap, uint32_t *out_len, int32_t *status, uint32_t *in_used,
-                               size_t n, size_t out_extent, bool count_only = false, uint32_t hist = 0) {
+                               size_t n, size_t out_extent, bool count_only = false, uint32_t hist = 0,
+                               const uint32_t *unit_hist = nullptr) {
   MetaLayout ml(n);
   CU(g.h_meta.reserve(ml.bytes));
   CU(g.d_meta.reserve(ml.bytes));
@@ -245,6 +267,10 @@ static int run_batch_on_staged(const uint64_t *in_off, const uint32_t *in_len, c
   memcpy(hm + ml.off_in_len, in_len, 4 * n);
   memcpy(hm + ml.off_out_cap, out_cap, 4 * n);
   CU(cudaMemcpyAsync(g.d_meta.p, hm, ml.inputs_bytes(), cudaMemcpyHostToDevice, g.stream));
+  if (unit_hist) {
+    memcpy(hm + ml.off_hist, unit_hist, 4 * n);
+    CU(cudaMemcpyAsync((uint8_t *)g.d_meta.p + ml.off_hist, hm + ml.off_hist, 4 * n, cudaMemcpyHostToDevice, g.stream));
+  }
   const size_t ws = workspace_bytes(n, out_extent);
   CU(g.d_ws.reserve(ws));
   uint8_t *dm = (uint8_t *)g.d_meta.p;
@@ -261,9 +287,10 @@ static int run_batch_on_staged(const uint64_t *in_off, const uint32_t *in_len, c
   b.n_units = n;
   b.ws = inflate_ws_carve(g.d_ws.p, n, out_extent);
   b.ws.hist = hist;
+  if (unit_hist) b.ws.unit_hist = (const uint32_t *)(dm + ml.off_hist);
   b.count_only = count_only;
   CU(launch_inflate(b, g.stream));
-  CU(cudaMemcpyAsync(hm + ml.off_out_len, dm + ml.off_out_len, ml.bytes - ml.off_out_len, cudaMemcpyDeviceToHost,
+  CU(cudaMemcpyAsync(hm + ml.off_out_len, dm + ml.off_out_len, ml.off_hist - ml.off_out_len, cudaMemcpyDeviceToHost,
                      g.stream));
   CU(cudaStreamSynchronize(g.stream));
   memcpy(out_len, hm + ml.off_out_len, 4 * n);
@@ -841,6 +868,139 @@ static bool gzip_member_header_within(const uint8_t *in, size_t n, size_t from, 
   return false;
 }
 
+// ---------------------------------------------------------------------------------------------
+// The rules that turn one unit's result into the next step of a gzip member loop or a zlib stream loop.  The single calls
+// (gzip_decode_staged, gzip_fast_path, zlib_decode_staged) and the batch driver (gzip_zlib_decode_streams) apply these.
+// ---------------------------------------------------------------------------------------------
+// The members of a hinted run whose hints were exact, from the front: the prefix that is accepted.
+static size_t hinted_exact_prefix(const std::vector<HintedMember> &ms, const uint32_t *len, const int32_t *st, const uint32_t *used) {
+  size_t k = 0;
+  while (k < ms.size() && st[k] == B200Z_U_DONE && len[k] == ms[k].isize && ms[k].hdr_end + used[k] + 8 == ms[k].next) ++k;
+  return k;
+}
+
+// A hinted run whose ISIZE fields bring the output to `o` bytes: B200Z_OK, or B200Z_E_NOSPC when out_cap is short of it.
+static int gzip_hinted_room_rule(size_t o, size_t out_cap) {
+  if (o <= out_cap) return B200Z_OK;
+  set_err("gzip_decode: output needs at least %zu bytes, out_cap %zu", o, out_cap);
+  return B200Z_E_NOSPC;
+}
+
+// The header of a member at `pos` that is decoded without a hint: 1 with *hdr_end = its DEFLATE stream, 0 when there is
+// no gzip header (the zlib loop goes on from `pos` on the same little-endian stream, :31-37), or B200Z_E_THROW.
+static int gzip_member_header_rule(const uint8_t *in, size_t in_len, size_t pos, size_t *hdr_end) {
+  size_t bsize;
+  const int h = gzip_header(in, in_len, pos, hdr_end, &bsize);
+  if (h >= 0) return h;
+  set_err("gzip_decode: truncated header (Dart: RangeError)");
+  return B200Z_E_THROW;
+}
+
+// The member at `pos` without a (valid) hint, its DEFLATE stream from hdr_end, came back as r: B200Z_OK with *next = where
+// the next member starts, or the call's result code.
+static int gzip_member_rule(const OneResult &r, size_t pos, size_t hdr_end, size_t in_len, size_t out_cap, size_t *next) {
+  if (r.status == B200Z_U_NOSPC) {
+    set_err("gzip_decode: out_cap %zu too small", out_cap);
+    return B200Z_E_NOSPC;
+  }
+  if (r.status == B200Z_U_RANGE || r.status == B200Z_U_THROW) {
+    set_err("gzip_decode: member at %zu: Dart would throw RangeError (status %d)", pos, r.status);
+    return B200Z_E_THROW;
+  }
+  const size_t after = hdr_end + r.in_used;
+  if (r.status == B200Z_U_STOP && after + 8 > in_len) {
+    // Inflate gave up because the input ran out inside a block (inflate.dart:166-168, 192-195): the byte-wise bit reader
+    // has pulled every byte by then, so the two readUint32 of the trailer (:40-41) start past the end -- RangeError.
+    // This is what a truncated file does.
+    set_err("gzip_decode: member at %zu: input ends inside the stream (Dart: RangeError)", pos);
+    return B200Z_E_THROW;
+  }
+  if (r.status != B200Z_U_DONE && r.status != B200Z_U_EOS) {
+    set_err("gzip_decode: member at %zu stopped with status %d", pos, r.status);
+    return B200Z_E_DATA;  // DESIGN.md "Divergences": reference keeps parsing from an unspecified position
+  }
+  if (after + 8 > in_len) {  // readUint32 x2 past the end (:40-41)
+    set_err("gzip_decode: truncated trailer (Dart: RangeError)");
+    return B200Z_E_THROW;
+  }
+  *next = after + 8;
+  return B200Z_OK;
+}
+
+// The zlib stream header at *pos (_zlib_decoder_web.dart:50-80): B200Z_OK with *pos behind it, or the call's result code.
+static int zlib_header_rule(const uint8_t *in, size_t in_len, size_t *pos) {
+  size_t p = *pos;
+  if (p + 2 > in_len) {
+    set_err("zlib_decode: truncated header (Dart: RangeError)");
+    return B200Z_E_THROW;
+  }
+  uint32_t cmf = in[p], flg = in[p + 1];
+  p += 2;
+  if ((cmf & 8) != 8) {  // :57 (sic)
+    set_err("zlib_decode: method != deflate");
+    return B200Z_E_DATA;
+  }
+  if (((cmf * 256) + flg) % 31 != 0) {
+    set_err("zlib_decode: bad FCHECK");
+    return B200Z_E_DATA;
+  }
+  if ((flg & 32) != 0) {
+    if (p + 4 > in_len) {
+      set_err("zlib_decode: truncated DICTID (Dart: RangeError)");
+      return B200Z_E_THROW;
+    }
+    set_err("zlib_decode: FDICT not supported");
+    return B200Z_E_DATA;
+  }
+  *pos = p;
+  return B200Z_OK;
+}
+
+// The zlib stream decoded from *pos came back as r, behind `committed` bytes of output: B200Z_OK with *pos behind the
+// stream and its Adler-32 field in *stored (not raw), or the call's result code with *out_len_total where it ends.
+static int zlib_stream_rule(const OneResult &r, const uint8_t *in, size_t in_len, int raw, int big_endian, size_t committed,
+                            size_t out_cap, size_t *pos, uint32_t *stored, size_t *out_len_total) {
+  if (r.status == B200Z_U_NOSPC) {
+    *out_len_total = committed + r.out_len;
+    set_err("zlib_decode: out_cap %zu too small", out_cap);
+    return B200Z_E_NOSPC;
+  }
+  if (r.status == B200Z_U_RANGE || r.status == B200Z_U_THROW) {
+    set_err("zlib_decode: Dart would throw RangeError (status %d)", r.status);
+    return B200Z_E_THROW;
+  }
+  if (r.status == B200Z_U_BADCODE) {
+    *out_len_total = committed + r.out_len;
+    set_err("zlib_decode: unusable Huffman code set");
+    return B200Z_E_DATA;
+  }
+  size_t p = *pos + r.in_used;
+  if (r.status == B200Z_U_STOP && p < in_len) {
+    // Inflate gave up with input left: the reference's stream position is then wherever its byte-wise bit buffer had
+    // got to (not rewound) -- unspecified; stop here with the partial output (DESIGN.md "Divergences").
+    *out_len_total = committed + r.out_len;
+    set_err("zlib_decode: inflate stopped early");
+    return B200Z_E_DATA;
+  }
+  // (B200Z_U_STOP with the input used up == the stream ends inside a block: Inflate simply returns what it has, :85)
+  if (!raw) {
+    if (p + 4 > in_len) {  // readUint32 past the end (:88); the stream's bytes were not handed over yet
+      set_err("zlib_decode: truncated Adler-32 (Dart: RangeError)");
+      return B200Z_E_THROW;
+    }
+    *stored = big_endian ? ((uint32_t)in[p] << 24 | in[p + 1] << 16 | in[p + 2] << 8 | in[p + 3]) : le32(in + p);
+    p += 4;
+  }
+  *pos = p;
+  return B200Z_OK;
+}
+
+static int zlib_adler_rule(uint32_t computed, uint32_t stored) {
+  if (computed == stored) return B200Z_OK;
+  set_err("zlib_decode: Adler-32 mismatch");
+  return B200Z_E_DATA;  // this stream's bytes are dropped (:91-94)
+}
+
 // GZip member loop on staged input.
 static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size_t out_cap, size_t *out_len_total,
                               size_t pos = 0, size_t out_pos = 0) {
@@ -852,23 +1012,20 @@ static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size
     // -------- gather a run of members that carry a size hint (BGZF 'BC' + ISIZE) --------
     v_in_off.clear(); v_out_off.clear(); v_in_len.clear(); v_out_cap.clear(); v_next.clear();
     size_t o = out_pos;
-    {
-      std::vector<HintedMember> run;
-      hinted_run(in, in_len, pos, &run, nullptr);
-      for (const HintedMember &m : run) {
-        v_in_off.push_back(m.hdr_end);
-        v_in_len.push_back((uint32_t)(m.next - m.hdr_end));
-        v_out_off.push_back(o);
-        v_out_cap.push_back(m.isize);
-        v_next.push_back(m.next);
-        o += m.isize;
-      }
+    std::vector<HintedMember> run;
+    hinted_run(in, in_len, pos, &run, nullptr);
+    for (const HintedMember &m : run) {
+      v_in_off.push_back(m.hdr_end);
+      v_in_len.push_back((uint32_t)(m.next - m.hdr_end));
+      v_out_off.push_back(o);
+      v_out_cap.push_back(m.isize);
+      v_next.push_back(m.next);
+      o += m.isize;
     }
     size_t nb = v_in_off.size();
     if (nb > 0) {
-      if (o > out_cap) {
+      if (gzip_hinted_room_rule(o, out_cap)) {
         *out_len_total = o;  // best knowledge of what is needed so far
-        set_err("gzip_decode: output needs at least %zu bytes, out_cap %zu", o, out_cap);
         return B200Z_E_NOSPC;
       }
       CU(g.d_out.reserve_keep(o + 64, out_pos, g.stream));
@@ -877,12 +1034,7 @@ static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size
                                    v_out_len.data(), v_status.data(), v_in_used.data(), nb, o);
       if (rc) return rc;
       // accept the prefix whose hints were exact; anything else is redone the slow, hint-free way
-      size_t k = 0;
-      for (; k < nb; ++k) {
-        bool ok = v_status[k] == B200Z_U_DONE && v_out_len[k] == v_out_cap[k] &&
-                  (size_t)v_in_off[k] + v_in_used[k] + 8 == v_next[k];
-        if (!ok) break;
-      }
+      const size_t k = hinted_exact_prefix(run, v_out_len.data(), v_status.data(), v_in_used.data());
       if (k > 0) {
         pos = v_next[k - 1];
         out_pos = v_out_off[k - 1] + v_out_len[k - 1];
@@ -891,12 +1043,11 @@ static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size
     }
     if (pos >= in_len) break;
     // -------- one member without (valid) hints: decode it alone to learn where it ends --------
-    size_t hdr_end, bsize;
-    int h = gzip_header(in, in_len, pos, &hdr_end, &bsize);
+    size_t hdr_end;
+    const int h = gzip_member_header_rule(in, in_len, pos, &hdr_end);
     if (h < 0) {
       *out_len_total = out_pos;
-      set_err("gzip_decode: truncated header (Dart: RangeError)");
-      return B200Z_E_THROW;
+      return h;
     }
     if (h == 0)  // no gzip header: fall back to zlib on the same little-endian stream (:31-37)
       return zlib_decode_staged(in, in_len, pos, verify & B200Z_GZIP_VERIFY, (verify & B200Z_GZIP_RAW) != 0, /*big_endian=*/0, out_pos,
@@ -909,31 +1060,8 @@ static int gzip_decode_staged(const uint8_t *in, size_t in_len, int verify, size
     if (rc) return rc;
     out_pos += r.out_len;
     *out_len_total = out_pos;
-    if (r.status == B200Z_U_NOSPC) {
-      set_err("gzip_decode: out_cap %zu too small", out_cap);
-      return B200Z_E_NOSPC;
-    }
-    if (r.status == B200Z_U_RANGE || r.status == B200Z_U_THROW) {
-      set_err("gzip_decode: member at %zu: Dart would throw RangeError (status %d)", pos, r.status);
-      return B200Z_E_THROW;
-    }
-    size_t after = hdr_end + r.in_used;
-    if (r.status == B200Z_U_STOP && after + 8 > in_len) {
-      // Inflate gave up because the input ran out inside a block (inflate.dart:166-168, 192-195): the byte-wise bit reader
-      // has pulled every byte by then, so the two readUint32 of the trailer (:40-41) start past the end -- RangeError.
-      // This is what a truncated file does.
-      set_err("gzip_decode: member at %zu: input ends inside the stream (Dart: RangeError)", pos);
-      return B200Z_E_THROW;
-    }
-    if (r.status != B200Z_U_DONE && r.status != B200Z_U_EOS) {
-      set_err("gzip_decode: member at %zu stopped with status %d", pos, r.status);
-      return B200Z_E_DATA;  // DESIGN.md "Divergences": reference keeps parsing from an unspecified position
-    }
-    if (after + 8 > in_len) {  // readUint32 x2 past the end (:40-41)
-      set_err("gzip_decode: truncated trailer (Dart: RangeError)");
-      return B200Z_E_THROW;
-    }
-    pos = after + 8;
+    rc = gzip_member_rule(r, pos, hdr_end, in_len, out_cap, &pos);
+    if (rc) return rc;
   }
   *out_len_total = out_pos;
   return B200Z_OK;
@@ -965,9 +1093,8 @@ static int gzip_fast_path(const uint8_t *in, size_t in_len, uint8_t *out, size_t
   const size_t o = *out_pos_io + promised;
   const size_t nb = ms.size();
   if (nb == 0) return B200Z_OK;
-  if (o > out_cap) {
+  if (gzip_hinted_room_rule(o, out_cap)) {
     *needed = o;
-    set_err("gzip_decode: output needs at least %zu bytes, out_cap %zu", o, out_cap);
     return B200Z_E_NOSPC;
   }
   const size_t in_lo = *pos_io, in_hi = p, out_lo = *out_pos_io;
@@ -1062,7 +1189,7 @@ static int gzip_fast_path(const uint8_t *in, size_t in_len, uint8_t *out, size_t
     const size_t ob = chunk_out_lo[c + 1] - chunk_out_lo[c];
     if (ob) CU(cudaMemcpyAsync(out + chunk_out_lo[c], (uint8_t *)g.d_out.p + chunk_out_lo[c], ob, cudaMemcpyDeviceToHost, g.s_d2h));
   }
-  CU(cudaMemcpyAsync(hm + ml.off_out_len, dm + ml.off_out_len, ml.bytes - ml.off_out_len, cudaMemcpyDeviceToHost, g.s_d2h));
+  CU(cudaMemcpyAsync(hm + ml.off_out_len, dm + ml.off_out_len, ml.off_hist - ml.off_out_len, cudaMemcpyDeviceToHost, g.s_d2h));
   CU(cudaStreamSynchronize(g.s_d2h));
   for (size_t c = 0; c < nchunks; ++c) {
     cudaEventDestroy(ev_in[c]);
@@ -1070,11 +1197,7 @@ static int gzip_fast_path(const uint8_t *in, size_t in_len, uint8_t *out, size_t
   }
   const uint32_t *r_len = (const uint32_t *)(hm + ml.off_out_len), *r_used = (const uint32_t *)(hm + ml.off_in_used);
   const int32_t *r_st = (const int32_t *)(hm + ml.off_status);
-  size_t k = 0;
-  for (; k < nb; ++k) {
-    bool ok = r_st[k] == B200Z_U_DONE && r_len[k] == ms[k].isize && ms[k].hdr_end + r_used[k] + 8 == ms[k].next;
-    if (!ok) break;
-  }
+  const size_t k = hinted_exact_prefix(ms, r_len, r_st, r_used);
   if (k > 0) {
     *pos_io = ms[k - 1].next;
     size_t oo = out_lo;
@@ -1217,17 +1340,13 @@ static int gzip_fast_path_piped(const uint8_t *in, size_t in_len, uint8_t *out, 
   if (rc) return rc;
   if (nospc) {
     *needed = promised;
-    set_err("gzip_decode: output needs at least %zu bytes, out_cap %zu", promised, out_cap);
-    return B200Z_E_NOSPC;
+    return gzip_hinted_room_rule(promised, out_cap);
   }
   const uint32_t *r_len = (const uint32_t *)(hm + ml.off_out_len), *r_used = (const uint32_t *)(hm + ml.off_in_used);
   const int32_t *r_st = (const int32_t *)(hm + ml.off_status);
-  size_t k = 0, oo = out_lo;
-  for (; k < nb; ++k) {
-    const bool ok = r_st[k] == B200Z_U_DONE && r_len[k] == ms[k].isize && ms[k].hdr_end + r_used[k] + 8 == ms[k].next;
-    if (!ok) break;
-    oo += ms[k].isize;
-  }
+  const size_t k = hinted_exact_prefix(ms, r_len, r_st, r_used);
+  size_t oo = out_lo;
+  for (size_t i = 0; i < k; ++i) oo += ms[i].isize;
   if (k > 0) {
     *pos_io = ms[k - 1].next;
     *out_pos_io = oo;
@@ -1299,28 +1418,8 @@ static int zlib_decode_staged(const uint8_t *in, size_t in_len, size_t pos, int 
   *out_len_total = committed;
   while (pos < in_len) {
     if (!raw) {
-      if (pos + 2 > in_len) {
-        set_err("zlib_decode: truncated header (Dart: RangeError)");
-        return B200Z_E_THROW;
-      }
-      uint32_t cmf = in[pos], flg = in[pos + 1];
-      pos += 2;
-      if ((cmf & 8) != 8) {  // :57 (sic)
-        set_err("zlib_decode: method != deflate");
-        return B200Z_E_DATA;
-      }
-      if (((cmf * 256) + flg) % 31 != 0) {
-        set_err("zlib_decode: bad FCHECK");
-        return B200Z_E_DATA;
-      }
-      if ((flg & 32) != 0) {
-        if (pos + 4 > in_len) {
-          set_err("zlib_decode: truncated DICTID (Dart: RangeError)");
-          return B200Z_E_THROW;
-        }
-        set_err("zlib_decode: FDICT not supported");
-        return B200Z_E_DATA;
-      }
+      const int rc = zlib_header_rule(in, in_len, &pos);
+      if (rc) return rc;
     }
     committed += pending;  // output.writeBytes(buffer) (:82-84)
     pending = 0;
@@ -1328,50 +1427,354 @@ static int zlib_decode_staged(const uint8_t *in, size_t in_len, size_t pos, int 
     OneResult r;
     int rc = run_one_staged(in, pos, in_len, committed, out_cap, &r);
     if (rc) return rc;
-    if (r.status == B200Z_U_NOSPC) {
-      *out_len_total = committed + r.out_len;
-      set_err("zlib_decode: out_cap %zu too small", out_cap);
-      return B200Z_E_NOSPC;
-    }
-    if (r.status == B200Z_U_RANGE || r.status == B200Z_U_THROW) {
-      set_err("zlib_decode: Dart would throw RangeError (status %d)", r.status);
-      return B200Z_E_THROW;
-    }
-    if (r.status == B200Z_U_BADCODE) {
-      *out_len_total = committed + r.out_len;
-      set_err("zlib_decode: unusable Huffman code set");
-      return B200Z_E_DATA;
-    }
-    pos += r.in_used;
-    if (r.status == B200Z_U_STOP && pos < in_len) {
-      // Inflate gave up with input left: the reference's stream position is then wherever its byte-wise bit buffer had
-      // got to (not rewound) -- unspecified; stop here with the partial output (DESIGN.md "Divergences").
-      *out_len_total = committed + r.out_len;
-      set_err("zlib_decode: inflate stopped early");
-      return B200Z_E_DATA;
-    }
-    // (B200Z_U_STOP with the input used up == the stream ends inside a block: Inflate simply returns what it has, :85)
-    if (!raw) {
-      if (pos + 4 > in_len) {  // readUint32 past the end (:88); the stream's bytes were not handed over yet
-        set_err("zlib_decode: truncated Adler-32 (Dart: RangeError)");
-        return B200Z_E_THROW;
-      }
-      uint32_t stored = big_endian ? ((uint32_t)in[pos] << 24 | in[pos + 1] << 16 | in[pos + 2] << 8 | in[pos + 3])
-                                   : le32(in + pos);
-      pos += 4;
-      if (verify) {
-        uint32_t a;
-        rc = device_adler32((const uint8_t *)g.d_out.p + committed, r.out_len, &a);
-        if (rc) return rc;
-        if (a != stored) {
-          set_err("zlib_decode: Adler-32 mismatch");
-          return B200Z_E_DATA;  // this stream's bytes are dropped (:91-94)
-        }
-      }
+    uint32_t stored = 0;
+    rc = zlib_stream_rule(r, in, in_len, raw, big_endian, committed, out_cap, &pos, &stored, out_len_total);
+    if (rc) return rc;
+    if (!raw && verify) {
+      uint32_t a;
+      rc = device_adler32((const uint8_t *)g.d_out.p + committed, r.out_len, &a);
+      if (rc) return rc;
+      rc = zlib_adler_rule(a, stored);
+      if (rc) return rc;
     }
     pending = r.out_len;
   }
   *out_len_total = committed + pending;  // (:101-103)
+  return B200Z_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Many gzip / zlib streams in one call (b200z_gzip_decode_batch / b200z_zlib_decode_batch).  Every stream keeps the state of
+// its own member loop (gzip_decode_staged) or stream loop (zlib_decode_staged) and takes its steps by the same rules; what
+// changes is that the steps of all streams of a device group are decoded together.  Per round each live stream offers its
+// hinted run, or else its next member / zlib stream, whose input view runs to the end of its own stream; the units of all of
+// them are one inflate batch, after the large ones have been offered to one K12 batch.  A batch of single-member files is
+// one round; a stream of k unhinted members takes k rounds, as it takes k steps alone.  The single calls keep their own
+// paths (the hinted run of a single gzip call is pipelined through gzip_fast_path).
+// ---------------------------------------------------------------------------------------------
+constexpr size_t GZ_STAGE = 64u << 20;        // the pinned staging buffer of the decode batch's outputs (Ctx::h_stage)
+static uint32_t g_gzb_max_group = 0;          // test hook: streams per device group (0: the memory budget alone)
+static unsigned long long g_gzb_stats[6];     // last call: streams, groups, rounds, units, offered to K12, accepted by K12
+
+struct GzStream {
+  const uint8_t *h = nullptr;  // the caller's bytes of the stream
+  size_t len = 0, cap = 0;     // its length and out_cap
+  size_t din = 0, dout = 0;    // its first byte in g.d_in / its output slot in g.d_out
+  size_t slot = 0;             // the slot's bytes: min(cap, max_inflate_out(len))
+  bool zlib = false, raw = false, verify = false, big_endian = false, skip_hint = false;
+  bool live = true;
+  int rc = B200Z_OK;
+  size_t pos = 0, out_pos = 0;  // gzip: position and output so far; zlib: out_pos = committed
+  size_t pending = 0, out_len = 0;
+  // this round
+  int kind = 0;  // 1: hinted run, 2: unhinted member, 3: zlib stream
+  size_t u0 = 0, hdr_end = 0;
+  std::vector<HintedMember> ms;
+  void finish(int r, size_t n) {
+    rc = r;
+    out_len = n;
+    live = false;
+    kind = 0;  // (a finished stream has no unit in this or any later round)
+  }
+};
+
+// The room of a unit that starts at out_pos of a stream's slot with `il` compressed bytes (run_one_staged's)
+static uint32_t gz_unit_room(const GzStream &s, size_t out_pos, uint32_t il) {
+  size_t room = s.slot > out_pos ? s.slot - out_pos : 0;
+  room = std::min(room, max_inflate_out(il));
+  return (uint32_t)std::min<size_t>(room, 0xfffffff0u);
+}
+
+// Puts the next step of a stream that is in its zlib stream loop into the unit table, or finishes it.
+struct GzUnits {
+  std::vector<uint64_t> in_off, out_off;
+  std::vector<uint32_t> in_len, cap, hist;
+  void add(uint64_t io, uint32_t il, uint64_t oo, uint32_t oc, uint32_t h) {
+    in_off.push_back(io);
+    in_len.push_back(il);
+    out_off.push_back(oo);
+    cap.push_back(oc);
+    hist.push_back(h);
+  }
+  size_t size() const { return in_off.size(); }
+};
+static void gz_zlib_step(GzStream &s, GzUnits &u) {
+  if (s.pos >= s.len) return s.finish(B200Z_OK, s.out_pos + s.pending);  // (:101-103)
+  if (!s.raw) {
+    const int r = zlib_header_rule(s.h, s.len, &s.pos);
+    if (r) return s.finish(r, s.out_pos);
+  }
+  s.out_pos += s.pending;  // output.writeBytes(buffer) (:82-84)
+  s.pending = 0;
+  const size_t avail = s.len - s.pos;
+  const uint32_t il = (uint32_t)std::min<size_t>(avail, 0xfffffff0u);
+  s.kind = 3;
+  s.u0 = u.size();
+  u.add(s.din + s.pos, il, s.dout + s.out_pos, gz_unit_room(s, s.out_pos, il), 0);
+}
+static void gz_gzip_step(GzStream &s, GzUnits &u) {
+  if (s.pos >= s.len) return s.finish(B200Z_OK, s.out_pos);
+  if (!s.skip_hint) {
+    s.ms.clear();
+    size_t promised = 0;
+    hinted_run(s.h, s.len, s.pos, &s.ms, &promised);
+    if (!s.ms.empty()) {
+      const size_t o = s.out_pos + promised;
+      if (gzip_hinted_room_rule(o, s.cap)) return s.finish(B200Z_E_NOSPC, o);
+      s.kind = 1;
+      s.u0 = u.size();
+      size_t op = s.out_pos;
+      for (const HintedMember &m : s.ms) {
+        // a hint that lies can promise more than the slot holds (slot < cap): the member then gets what is left, fails
+        // its hint and is redone hint-free, as a lying hint is anyway
+        const uint32_t room = (uint32_t)std::min<size_t>(m.isize, s.slot > op ? s.slot - op : 0);
+        u.add(s.din + m.hdr_end, (uint32_t)(m.next - m.hdr_end), s.dout + op, room, 0);
+        op += m.isize;
+      }
+      return;
+    }
+  }
+  s.skip_hint = false;
+  const int h = gzip_member_header_rule(s.h, s.len, s.pos, &s.hdr_end);
+  if (h < 0) return s.finish(h, s.out_pos);
+  if (h == 0) {  // no gzip header: the zlib loop on the same little-endian stream (:31-37), from here on
+    s.zlib = true;
+    s.big_endian = false;
+    s.pending = 0;
+    return gz_zlib_step(s, u);
+  }
+  const uint32_t il = (uint32_t)std::min<size_t>(s.len - s.hdr_end, 0xfffffff0u);
+  s.kind = 2;
+  s.u0 = u.size();
+  u.add(s.din + s.hdr_end, il, s.dout + s.out_pos, gz_unit_room(s, s.out_pos, il),
+        (uint32_t)std::min<size_t>(s.out_pos, 65535));  // distances end at 32768
+}
+
+// One device group: streams [a, b) of `st`, whose inputs and slots are laid out from 0 in g.d_in / g.d_out.
+static int gz_decode_group(std::vector<GzStream> &st, size_t a, size_t b, size_t in_bytes, size_t out_bytes,
+                           const std::vector<uint8_t> &packed_in) {
+  CU(g.d_in.reserve(in_bytes + 64));
+  CU(g.d_out.reserve(out_bytes + 64));
+  if (in_bytes) CU(cudaMemcpyAsync(g.d_in.p, packed_in.data(), in_bytes, cudaMemcpyHostToDevice, g.stream));
+  g_gzb_stats[1]++;
+  GzUnits u;
+  std::vector<uint32_t> r_len, r_used;
+  std::vector<int32_t> r_st;
+  for (;;) {
+    u = GzUnits();
+    for (size_t i = a; i < b; ++i) {
+      GzStream &s = st[i];
+      if (!s.live) continue;
+      s.kind = 0;
+      if (s.zlib)
+        gz_zlib_step(s, u);
+      else
+        gz_gzip_step(s, u);
+    }
+    const size_t nu = u.size();
+    if (nu == 0) break;
+    g_gzb_stats[2]++;
+    g_gzb_stats[3] += nu;
+    r_len.assign(nu, 0);
+    r_used.assign(nu, 0);
+    r_st.assign(nu, 0);
+    std::vector<bool> done(nu, false);
+    // K12 first for the large units (run_one_staged's rule; a gzip member only when no successor header is near)
+    std::vector<CkIn> ck;
+    std::vector<size_t> ck_unit;
+    for (size_t i = a; i < b; ++i) {
+      const GzStream &s = st[i];
+      if (!s.live || (s.kind != 2 && s.kind != 3)) continue;
+      const size_t k = s.u0;
+      if (u.in_len[k] < g_ck.thresh) continue;
+      if (s.kind == 2 && gzip_member_header_within(s.h, s.len, s.hdr_end, g_ck.thresh)) continue;
+      const uint32_t n_pages = ck_pages_for(workspace_bytes(1, s.out_pos + u.cap[k]));
+      if (!n_pages) continue;
+      const size_t at = s.kind == 2 ? s.hdr_end : s.pos;
+      ck.push_back(CkIn{s.h + at, u.in_off[k], u.in_len[k], u.out_off[k], u.cap[k], u.hist[k], n_pages});
+      ck_unit.push_back(k);
+    }
+    if (!ck.empty()) {
+      std::vector<CkOut> res;
+      double ms[3] = {0, 0, 0};
+      const int rc = run_chunked(ck, res, ms);
+      if (rc) return rc;
+      g_gzb_stats[4] += ck.size();
+      for (size_t c = 0; c < ck.size(); ++c)
+        if (res[c].accepted) {
+          const size_t k = ck_unit[c];
+          r_len[k] = res[c].r.out_len;
+          r_used[k] = res[c].r.in_used;
+          r_st[k] = res[c].r.status;
+          done[k] = true;
+          g_gzb_stats[5]++;
+        }
+    }
+    // everything else: one inflate batch (k_inflate_fast first when no unit has a history)
+    {
+      GzUnits v;
+      std::vector<size_t> back;
+      bool any_hist = false;
+      for (size_t k = 0; k < nu; ++k)
+        if (!done[k]) {
+          v.add(u.in_off[k], u.in_len[k], u.out_off[k], u.cap[k], u.hist[k]);
+          back.push_back(k);
+          any_hist |= u.hist[k] != 0;
+        }
+      if (!back.empty()) {
+        const size_t m = back.size();
+        size_t extent = 0;
+        for (size_t k = 0; k < m; ++k) extent = std::max<size_t>(extent, v.out_off[k] + v.cap[k]);
+        std::vector<uint32_t> l(m), us(m);
+        std::vector<int32_t> sv(m);
+        const int rc = run_batch_on_staged(v.in_off.data(), v.in_len.data(), v.out_off.data(), v.cap.data(), l.data(), sv.data(),
+                                           us.data(), m, extent, false, 0, any_hist ? v.hist.data() : nullptr);
+        if (rc) return rc;
+        for (size_t k = 0; k < m; ++k) {
+          r_len[back[k]] = l[k];
+          r_used[back[k]] = us[k];
+          r_st[back[k]] = sv[k];
+        }
+      }
+    }
+    // each stream's next step, by the rules of the single calls
+    std::vector<size_t> ad_stream;
+    std::vector<uint64_t> ad_off, ad_len;
+    std::vector<uint32_t> ad_stored;
+    for (size_t i = a; i < b; ++i) {
+      GzStream &s = st[i];
+      if (!s.live || s.kind == 0) continue;
+      const size_t k = s.u0;
+      if (s.kind == 1) {
+        const size_t acc = hinted_exact_prefix(s.ms, &r_len[k], &r_st[k], &r_used[k]);
+        size_t op = s.out_pos;
+        for (size_t j = 0; j < acc; ++j) op += s.ms[j].isize;
+        if (acc > 0) s.pos = s.ms[acc - 1].next;
+        s.out_pos = op;
+        s.skip_hint = acc < s.ms.size();
+        continue;
+      }
+      const OneResult r{r_len[k], r_used[k], r_st[k]};
+      if (s.kind == 2) {
+        s.out_pos += r.out_len;
+        const int rc = gzip_member_rule(r, s.pos, s.hdr_end, s.len, s.cap, &s.pos);
+        if (rc) s.finish(rc, s.out_pos);
+        continue;
+      }
+      uint32_t stored = 0;
+      size_t n = s.out_pos;
+      const int rc = zlib_stream_rule(r, s.h, s.len, s.raw, s.big_endian, s.out_pos, s.cap, &s.pos, &stored, &n);
+      if (rc) {
+        s.finish(rc, n);
+        continue;
+      }
+      s.pending = r.out_len;
+      if (!s.raw && s.verify) {
+        ad_stream.push_back(i);
+        ad_off.push_back(s.dout + s.out_pos);
+        ad_len.push_back(r.out_len);
+        ad_stored.push_back(stored);
+      }
+    }
+    if (!ad_stream.empty()) {  // one Adler-32 launch for every stream of the round that finished a zlib stream
+      std::vector<uint32_t> ad(ad_stream.size());
+      const int rc = device_adler32_many((const uint8_t *)g.d_out.p, ad_off.data(), ad_len.data(), ad_stream.size(), ad.data());
+      if (rc) return rc;
+      for (size_t j = 0; j < ad_stream.size(); ++j) {
+        GzStream &s = st[ad_stream[j]];
+        if (zlib_adler_rule(ad[j], ad_stored[j])) s.finish(B200Z_E_DATA, s.out_pos);
+      }
+    }
+  }
+  return B200Z_OK;
+}
+
+// n streams (arguments checked): rc[i] / out_len[i] / the slot's bytes as b200z_gzip_decode (gzip) or b200z_zlib_decode
+// give for stream i alone; `verify` takes B200Z_GZIP_VERIFY / B200Z_GZIP_RAW for gzip, a bool for zlib
+static int gzip_zlib_decode_streams(bool gzip, const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                                    int verify, int raw, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                    uint64_t *out_len, int32_t *rc) {
+  for (auto &v : g_gzb_stats) v = 0;
+  g_gzb_stats[0] = n;
+  std::vector<GzStream> st(n);
+  for (size_t i = 0; i < n; ++i) {
+    GzStream &s = st[i];
+    s.h = in_len[i] ? in_base + in_off[i] : nullptr;
+    s.len = (size_t)in_len[i];
+    s.cap = (size_t)out_cap[i];
+    s.slot = std::min<size_t>(s.cap, max_inflate_out(s.len));
+    if (gzip) {
+      s.verify = (verify & B200Z_GZIP_VERIFY) != 0;
+      s.raw = (verify & B200Z_GZIP_RAW) != 0;
+    } else {
+      s.zlib = true;
+      s.verify = verify != 0;
+      s.raw = raw != 0;
+      s.big_endian = true;
+    }
+  }
+  // device groups: consecutive streams whose inputs, slots and inflate workspace fit half the free device memory
+  size_t budget = (size_t)32 << 30;
+  {
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b)
+      budget = std::min(budget, (free_b + g.d_in.cap + g.d_out.cap + g.d_ws.cap) / 2);
+  }
+  std::vector<uint8_t> packed;
+  size_t a = 0;
+  while (a < n) {
+    size_t b = a, in_bytes = 0, out_bytes = 0;
+    while (b < n) {
+      const size_t ib = align_up(st[b].len + 64, 256), ob = align_up(st[b].slot + 64, 256);
+      const size_t need = in_bytes + ib + out_bytes + ob + workspace_bytes(b - a + 1, out_bytes + ob);
+      if (b > a && (need > budget || (g_gzb_max_group && b - a >= g_gzb_max_group))) break;
+      st[b].din = in_bytes;
+      st[b].dout = out_bytes;
+      in_bytes += ib;
+      out_bytes += ob;
+      ++b;
+    }
+    // the group's inputs, each followed by zeros up to the next, go up in one copy
+    packed.assign(in_bytes, 0);
+    for (size_t i = a; i < b; ++i)
+      if (st[i].len) memcpy(packed.data() + st[i].din, st[i].h, st[i].len);
+    int r = gz_decode_group(st, a, b, in_bytes, out_bytes, packed);
+    if (r) return r;
+    // results, and the bytes of every stream that did not run out of room (the single calls copy nothing then).  The
+    // bytes come back through a pinned staging buffer of at most GZ_STAGE bytes, one asynchronous copy per stream and one
+    // synchronise per fill; a stream larger than the buffer is copied straight into its slot.
+    size_t i0 = a, o = 0;
+    auto drain = [&](size_t i1) -> int {  // streams [i0, i1) are in the staging buffer, back to back
+      CU(cudaStreamSynchronize(g.stream));
+      for (size_t p = 0; i0 < i1; ++i0) {
+        const size_t k = st[i0].rc == B200Z_E_NOSPC ? 0 : std::min(st[i0].out_len, st[i0].cap);
+        if (k && k <= GZ_STAGE) {
+          memcpy(out_base + out_off[i0], (const uint8_t *)g.h_stage.p + p, k);
+          p += k;
+        }
+      }
+      o = 0;
+      return B200Z_OK;
+    };
+    for (size_t i = a; i < b; ++i) {
+      const size_t k = st[i].rc == B200Z_E_NOSPC ? 0 : std::min(st[i].out_len, st[i].cap);
+      const uint8_t *src = (const uint8_t *)g.d_out.p + st[i].dout;
+      if (k > GZ_STAGE) {
+        CU(cudaMemcpyAsync(out_base + out_off[i], src, k, cudaMemcpyDeviceToHost, g.stream));
+      } else if (k) {
+        if (o + k > GZ_STAGE && (r = drain(i)) != B200Z_OK) return r;
+        CU(g.h_stage.reserve(GZ_STAGE));
+        CU(cudaMemcpyAsync((uint8_t *)g.h_stage.p + o, src, k, cudaMemcpyDeviceToHost, g.stream));
+        o += k;
+      }
+    }
+    if ((r = drain(b)) != B200Z_OK) return r;
+    for (size_t i = a; i < b; ++i) {
+      out_len[i] = st[i].out_len;
+      rc[i] = st[i].rc;
+    }
+    a = b;
+  }
   return B200Z_OK;
 }
 
@@ -2151,9 +2554,10 @@ static int deflate_member_on(const uint8_t *d_in, size_t n, int level, int windo
   return device_crc32_on(d_in, n, (uint32_t *)ws, s, crc);
 }
 
+// adler32, when given: every input's Adler-32 as well, from one launch over the staged inputs
 static int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n_units, int level,
                               int window_bits, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
-                              uint64_t *out_len, uint32_t *crc32, int32_t *status) {
+                              uint64_t *out_len, uint32_t *crc32, int32_t *status, uint32_t *adler32 = nullptr) {
   std::vector<size_t> din(n_units + 1), dout(n_units + 1);
   size_t ws_lane = 4096, acc_in = 0, acc_out = 0;
   for (size_t i = 0; i < n_units; ++i) {
@@ -2307,6 +2711,84 @@ static int deflate_batch_impl(const uint8_t *in_base, const uint64_t *in_off, co
       set_err("deflate_batch: %s", lane_err[l].empty() ? "a lane failed" : lane_err[l].c_str());
       return lane_rc[l];
     }
+  if (adler32) {
+    const std::vector<uint64_t> off(din.begin(), din.end() - 1);
+    return device_adler32_many((const uint8_t *)g.d_in.p, off.data(), in_len, n_units, adler32);
+  }
+  return B200Z_OK;
+}
+
+// The framing GZipEncoder / ZLibEncoder write around the DEFLATE bytes.  Header (_gzip_encoder_web.dart:77-90): magic,
+// deflate, flags 0, MTIME, XFL 0, OS 255; trailer: CRC-32 and ISIZE, little-endian.
+static void gzip_put_header(uint8_t *o, uint32_t mtime) {
+  o[0] = 0x1f; o[1] = 0x8b; o[2] = 8; o[3] = 0;
+  for (int i = 0; i < 4; ++i) o[4 + i] = (uint8_t)(mtime >> (8 * i));
+  o[8] = 0; o[9] = 255;
+}
+static void gzip_put_trailer(uint8_t *o, uint32_t crc, size_t n) {
+  for (int i = 0; i < 4; ++i) o[i] = (uint8_t)(crc >> (8 * i));
+  for (int i = 0; i < 4; ++i) o[4 + i] = (uint8_t)((uint32_t)n >> (8 * i));
+}
+// CMF / FLG with FLEVEL 0 for every level (_zlib_encoder_web.dart:44-60, quirk Q4); the Adler-32 behind is big-endian
+static void zlib_put_header(uint8_t *o, int window_bits) {
+  int wb = window_bits < 0 ? 0 : window_bits > 15 ? 15 : window_bits;
+  int cmf = ((wb - 8) << 4) | 8, flag = 0, fcheck = 0;
+  while ((cmf * 256 + (flag | fcheck)) % 31 != 0) fcheck++;
+  o[0] = (uint8_t)cmf;
+  o[1] = (uint8_t)(flag | fcheck);
+}
+static void zlib_put_adler(uint8_t *o, uint32_t ad) {
+  o[0] = (uint8_t)(ad >> 24); o[1] = (uint8_t)(ad >> 16); o[2] = (uint8_t)(ad >> 8); o[3] = (uint8_t)ad;
+}
+
+// n inputs (arguments, level and windowBits checked) encoded as b200z_gzip_encode (gzip) or b200z_zlib_encode give each
+// alone: one deflate batch whose raw DEFLATE goes behind the header inside each slot; CRC-32 from the batch, Adler-32 from
+// one launch; the host writes the headers and trailers.
+static int gzip_zlib_encode_streams(bool gzip, const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                                    int level, int window_bits, int raw, uint32_t mtime, uint8_t *out_base,
+                                    const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  const size_t hdr = gzip ? 10 : raw ? 0 : 2, trl = gzip ? 8 : raw ? 0 : 4;
+  std::vector<size_t> idx;
+  for (size_t i = 0; i < n; ++i) {
+    if (in_len[i] >= 0xffff0000ull) {  // deflate_staged's limit
+      rc[i] = B200Z_E_ARG;
+      out_len[i] = 0;
+    } else {
+      idx.push_back(i);
+    }
+  }
+  const size_t m = idx.size();
+  if (m == 0) return B200Z_OK;
+  std::vector<uint64_t> io(m), il(m), oo(m), oc(m), ol(m);
+  std::vector<uint32_t> crc(m), ad(m);
+  std::vector<int32_t> st(m);
+  for (size_t k = 0; k < m; ++k) {
+    const size_t i = idx[k];
+    io[k] = in_off[i];
+    il[k] = in_len[i];
+    oo[k] = out_off[i] + hdr;
+    oc[k] = out_cap[i] >= hdr + trl ? out_cap[i] - hdr - trl : 0;
+  }
+  const int r = deflate_batch_impl(in_base, io.data(), il.data(), m, level, window_bits, out_base, oo.data(), oc.data(), ol.data(),
+                                   crc.data(), st.data(), !gzip && !raw ? ad.data() : nullptr);
+  if (r) return r;
+  for (size_t k = 0; k < m; ++k) {
+    const size_t i = idx[k];
+    out_len[i] = ol[k] + hdr + trl;
+    if (st[k] != B200Z_OK) {
+      rc[i] = B200Z_E_NOSPC;
+      continue;
+    }
+    uint8_t *o = out_base + out_off[i];
+    if (gzip) {
+      gzip_put_header(o, mtime);
+      gzip_put_trailer(o + hdr + ol[k], crc[k], (size_t)il[k]);
+    } else if (!raw) {
+      zlib_put_header(o, window_bits);
+      zlib_put_adler(o + hdr + ol[k], ad[k]);
+    }
+    rc[i] = B200Z_OK;
+  }
   return B200Z_OK;
 }
 
@@ -3635,7 +4117,7 @@ void b200z_shutdown(void) {
   cudaSetDevice(g.device);
   cudaStreamSynchronize(g.stream);
   g.d_in.release(); g.d_out.release(); g.d_ws.release(); g.d_meta.release(); g.d_small.release(); g.d_bz.release(); g.d_tok.release(); g.d_crypt.release();
-  g.h_meta.release();
+  g.h_meta.release(); g.h_stage.release();
   cudaStreamDestroy(g.stream);
   cudaStreamDestroy(g.s_h2d);
   cudaStreamDestroy(g.s_d2h);
@@ -3805,12 +4287,8 @@ int b200z_zlib_encode(const uint8_t *in, size_t in_len, int level, int window_bi
   }
   size_t o = 0;
   if (!raw) {
-    // CMF / FLG with FLEVEL 0 for every level (_zlib_encoder_web.dart:44-60, quirk Q4)
-    int wb = window_bits < 0 ? 0 : window_bits > 15 ? 15 : window_bits;
-    int cmf = ((wb - 8) << 4) | 8, flag = 0, fcheck = 0;
-    while ((cmf * 256 + (flag | fcheck)) % 31 != 0) fcheck++;
-    out[o++] = (uint8_t)cmf;
-    out[o++] = (uint8_t)(flag | fcheck);
+    zlib_put_header(out, window_bits);
+    o = 2;
   }
   if (n) CU(cudaMemcpyAsync(out + o, g.d_out.p, n, cudaMemcpyDeviceToHost, g.stream));
   o += n;
@@ -3818,10 +4296,7 @@ int b200z_zlib_encode(const uint8_t *in, size_t in_len, int level, int window_bi
     uint32_t ad;
     rc = device_adler32((const uint8_t *)g.d_in.p, in_len, &ad);
     if (rc) return rc;
-    out[o++] = (uint8_t)(ad >> 24);
-    out[o++] = (uint8_t)(ad >> 16);
-    out[o++] = (uint8_t)(ad >> 8);
-    out[o++] = (uint8_t)ad;
+    zlib_put_adler(out + o, ad);
   }
   CU(cudaStreamSynchronize(g.stream));
   return B200Z_OK;
@@ -3845,18 +4320,12 @@ int b200z_gzip_encode(const uint8_t *in, size_t in_len, int level, uint32_t mtim
     set_err("gzip_encode: output needs %zu bytes, out_cap %zu", total, out_cap);
     return B200Z_E_NOSPC;
   }
-  // header (_gzip_encoder_web.dart:77-90): magic, deflate, flags 0, MTIME, XFL 0, OS 255
-  size_t o = 0;
-  out[o++] = 0x1f; out[o++] = 0x8b; out[o++] = 8; out[o++] = 0;
-  for (int i = 0; i < 4; ++i) out[o++] = (uint8_t)(mtime >> (8 * i));
-  out[o++] = 0; out[o++] = 255;
-  if (n) CU(cudaMemcpyAsync(out + o, g.d_out.p, n, cudaMemcpyDeviceToHost, g.stream));
-  o += n;
+  gzip_put_header(out, mtime);
+  if (n) CU(cudaMemcpyAsync(out + 10, g.d_out.p, n, cudaMemcpyDeviceToHost, g.stream));
   uint32_t crc;
   rc = device_crc32((const uint8_t *)g.d_in.p, in_len, &crc);
   if (rc) return rc;
-  for (int i = 0; i < 4; ++i) out[o++] = (uint8_t)(crc >> (8 * i));
-  for (int i = 0; i < 4; ++i) out[o++] = (uint8_t)((uint32_t)in_len >> (8 * i));
+  gzip_put_trailer(out + 10 + n, crc, in_len);
   CU(cudaStreamSynchronize(g.stream));
   return B200Z_OK;
 }
@@ -3912,6 +4381,65 @@ int b200z_zlib_decode(const uint8_t *in, size_t in_len, int verify, int raw, uin
   if (n) CU(cudaMemcpyAsync(out, g.d_out.p, n, cudaMemcpyDeviceToHost, g.stream));
   CU(cudaStreamSynchronize(g.stream));
   return rc;
+}
+
+int b200z_gzip_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                            uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  r = xz_batch_args("gzip_decode_batch", in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, rc);
+  if (r) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return gzip_zlib_decode_streams(true, in_base, in_off, in_len, n, verify, 0, out_base, out_off, out_cap, out_len, rc);
+}
+int b200z_zlib_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify, int raw,
+                            uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  r = xz_batch_args("zlib_decode_batch", in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, rc);
+  if (r) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return gzip_zlib_decode_streams(false, in_base, in_off, in_len, n, verify, raw, out_base, out_off, out_cap, out_len, rc);
+}
+int b200z_gzip_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int level,
+                            uint32_t mtime, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                            int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  if (level < 0 || level > 9) {
+    set_err("gzip_encode_batch: invalid level %d (Dart: LateInitializationError)", level);
+    return B200Z_E_ARG;
+  }
+  r = xz_batch_args("gzip_encode_batch", in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, rc);
+  if (r || n == 0) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return gzip_zlib_encode_streams(true, in_base, in_off, in_len, n, level, 15, 0, mtime, out_base, out_off, out_cap, out_len, rc);
+}
+int b200z_zlib_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int level,
+                            int window_bits, int raw, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                            uint64_t *out_len, int32_t *rc) {
+  int r = require_init();
+  if (r) return r;
+  if (window_bits < 9 || window_bits > 15 || level < 0 || level > 9) {
+    set_err("zlib_encode_batch: invalid level %d / windowBits %d (Dart: LateInitializationError)", level, window_bits);
+    return B200Z_E_ARG;
+  }
+  r = xz_batch_args("zlib_encode_batch", in_base, in_off, in_len, n, out_base, out_off, out_cap, out_len, rc);
+  if (r || n == 0) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  return gzip_zlib_encode_streams(false, in_base, in_off, in_len, n, level, window_bits, raw, 0, out_base, out_off, out_cap, out_len,
+                                  rc);
+}
+// (test hooks, not part of the ABI) cap on the streams of one gzip / zlib decode device group (0: the memory budget
+// alone); the last b200z_gzip_decode_batch / b200z_zlib_decode_batch call's streams, device groups, rounds, inflate units,
+// and units offered to / accepted by K12
+void b200z_debug_gzip_batch_set(unsigned max_streams) { g_gzb_max_group = max_streams; }
+void b200z_debug_gzip_batch_stats(unsigned long long out[6]) {
+  for (int k = 0; k < 6; ++k) out[k] = g_gzb_stats[k];
 }
 
 }  // extern "C"

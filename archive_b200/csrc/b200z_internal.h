@@ -33,6 +33,9 @@ struct InflateWs {
   // a member's distance may reach into the members before it (output_memory_stream.dart:79-98 checks against the whole
   // stream): the member-by-member path sets this for its single-unit batches.
   uint32_t hist = 0;
+  // The same per unit ([n_units], device memory) when the units of one batch have different histories (members of many
+  // gzip streams decoded together); it takes the place of `hist` when set.
+  const uint32_t *unit_hist = nullptr;
 };
 size_t inflate_ws_bytes(size_t n_units, size_t extent);
 // largest extent a workspace of `bytes` serves (extent 0 is valid); INFLATE_WS_TOO_SMALL when it serves none

@@ -29,6 +29,7 @@ struct InflateWs {
   uint32_t *pieces = nullptr;
   uint8_t *uscratch = nullptr;
   uint32_t hist = 0;
+  const uint32_t *unit_hist = nullptr;
 };
 }  // namespace b200z
 #else
@@ -55,8 +56,14 @@ namespace b200z {
 #define B200Z_DYN_SMEM(name) extern __shared__ __align__(16) uint32_t name[]
 #endif
 
-// HIST: the unit may reach InflateWs::hist bytes of earlier output (single gzip members decoded behind their predecessors).
-// The batch kernels are the HIST = false instantiations: the history term folds away and their code is what it was.
+// HIST: the unit may reach InflateWs::hist (or its own InflateWs::unit_hist entry) bytes of earlier output (gzip members
+// decoded behind their predecessors).  The batch kernels are the HIST = false instantiations: the history term folds away
+// and their code is what it was.
+template <bool HIST>
+__device__ __forceinline__ uint32_t unit_history(const InflateWs &ws, uint32_t unit) {
+  return HIST ? (ws.unit_hist ? ws.unit_hist[unit] : ws.hist) : 0u;
+}
+
 template <bool HIST>
 __global__ void __launch_bounds__(B200Z_DECODE_THREADS)
 k_inflate_decode(const uint8_t *__restrict__ in_base, const uint64_t *__restrict__ in_off,
@@ -106,9 +113,10 @@ k_inflate_decode(const uint8_t *__restrict__ in_base, const uint64_t *__restrict
   sc.hcap = 0;
   sc.bm = nullptr;
   sc.pieces = nullptr;
-  sc.hist = HIST ? ws.hist : 0u;
+  sc.hist = 0u;
   uint32_t *tok = nullptr;
   if (active) {
+    sc.hist = unit_history<HIST>(ws, unit);
     const uint64_t oo = out_off[unit];
     const uint32_t cap = out_cap[unit];
     tok = ws.tokens + oo;  // token region mirrors the output layout (<= 1 token per output byte)
@@ -152,7 +160,7 @@ k_inflate_expand(InflateWs ws, const uint8_t *__restrict__ in_base, const uint64
     // Positions below count from `hist` bytes in front of the unit (InflateWs::hist; 0 unless the unit is a gzip member
     // decoded on its own behind its predecessors): the range check, the capacity check and the source reads then need
     // nothing extra.
-    const uint32_t hist = HIST ? ws.hist : 0u;
+    const uint32_t hist = unit_history<HIST>(ws, unit);
     const uint32_t cap = HIST ? (out_cap[unit] > 0xffffffffu - hist ? 0xffffffffu : out_cap[unit] + hist) : out_cap[unit];
     const uint32_t *P = ws.pieces + (size_t)unit * PIECE_WORDS;
     const uint32_t np = P[0];
@@ -487,7 +495,7 @@ cudaError_t launch_inflate(const InflateBatch &b, cudaStream_t stream) {
     // token buffer in global memory (DESIGN.md K1f).
     const char *fe = getenv("B200Z_FAST");
     const int fast_on = fe ? atoi(fe) : 1;
-    if (fast_on && !b.count_only && b.ws.hist == 0 && b.ws.pieces != nullptr && b.ws.uscratch != nullptr) {
+    if (fast_on && !b.count_only && b.ws.hist == 0 && b.ws.unit_hist == nullptr && b.ws.pieces != nullptr && b.ws.uscratch != nullptr) {
       static uint64_t attr_done = 0;  // one bit per device: function attributes belong to the device's context
       if (!((attr_done >> (cur_dev & 63)) & 1u)) {
         cudaError_t e = cudaFuncSetAttribute(k_inflate_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fp::SMEM_BYTES);
@@ -516,7 +524,8 @@ cudaError_t launch_inflate(const InflateBatch &b, cudaStream_t stream) {
     }
   }
   if (g_prof) cudaEventRecord(pt.f, stream);
-  if (b.ws.hist)
+  const bool with_hist = b.ws.hist != 0 || b.ws.unit_hist != nullptr;
+  if (with_hist)
     k_inflate_decode<true><<<blocks, B200Z_DECODE_THREADS, smem, stream>>>(b.in_base, b.in_off, b.in_len, b.out_off, b.out_cap, b.ws,
                                                                          b.out_len, b.status, b.in_used, (uint32_t)b.n_units, upw,
                                                                          b.count_only ? 1 : lpu, b.count_only ? 1 : 0, after_fast);
@@ -546,7 +555,7 @@ cudaError_t launch_inflate(const InflateBatch &b, cudaStream_t stream) {
   }
   const uint64_t max_blocks = (uint64_t)g_num_sms * (uint64_t)bps;
   if (eblocks > max_blocks) eblocks = max_blocks;
-  if (b.ws.hist)
+  if (with_hist)
     k_inflate_expand<true><<<(unsigned)eblocks, B200Z_EXPAND_THREADS, 0, stream>>>(b.ws, b.in_base, b.in_off, b.out_base, b.out_off,
                                                                                  b.out_cap, b.out_len, b.status, (uint32_t)b.n_units, after_fast);
   else

@@ -43,6 +43,27 @@ typedef _Bz2DecodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64>
     Int32 verify, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Int32> rc);
 typedef _Bz2DecodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
     int verify, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Int32> rc);
+// b200z_zlib_decode_batch: (inBase, inOff, inLen, n, verify, raw, outBase, outOff, outCap, outLen, rc)
+typedef _ZlibDecodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Int32 verify, Int32 raw, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc);
+typedef _ZlibDecodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    int verify, int raw, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc);
+// b200z_gzip_encode_batch: (inBase, inOff, inLen, n, level, mtime, outBase, outOff, outCap, outLen, rc)
+typedef _GzipEncodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Int32 level, Uint32 mtime, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap,
+    Pointer<Uint64> outLen, Pointer<Int32> rc);
+typedef _GzipEncodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    int level, int mtime, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc);
+// b200z_zlib_encode_batch: (inBase, inOff, inLen, n, level, windowBits, raw, outBase, outOff, outCap, outLen, rc)
+typedef _ZlibEncodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Int32 level, Int32 windowBits, Int32 raw, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap,
+    Pointer<Uint64> outLen, Pointer<Int32> rc);
+typedef _ZlibEncodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    int level, int windowBits, int raw, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap,
+    Pointer<Uint64> outLen, Pointer<Int32> rc);
 typedef _Bz2EncodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
     Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen, Pointer<Uint32> crc32,
     Pointer<Int32> rc);
@@ -271,6 +292,15 @@ class B200Z {
       _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_xz_decode_batch');
   late final _Bz2DecodeBatchD xzEncodeBatch =
       _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_xz_encode_batch');
+  // gzip / zlib batches: gzip decode has the shape of b200z_bzip2_decode_batch (verify = B200Z_GZIP_VERIFY | _RAW bits)
+  late final _Bz2DecodeBatchD gzipDecodeBatch =
+      _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_gzip_decode_batch');
+  late final _ZlibDecodeBatchD zlibDecodeBatch =
+      _lib.lookupFunction<_ZlibDecodeBatchC, _ZlibDecodeBatchD>('b200z_zlib_decode_batch');
+  late final _GzipEncodeBatchD gzipEncodeBatch =
+      _lib.lookupFunction<_GzipEncodeBatchC, _GzipEncodeBatchD>('b200z_gzip_encode_batch');
+  late final _ZlibEncodeBatchD zlibEncodeBatch =
+      _lib.lookupFunction<_ZlibEncodeBatchC, _ZlibEncodeBatchD>('b200z_zlib_encode_batch');
   late final _DeflateBatchD deflateBatch = _lib.lookupFunction<_DeflateBatchC, _DeflateBatchD>('b200z_deflate_batch');
   late final _InflateBatchD inflateBatch = _lib.lookupFunction<_InflateBatchC, _InflateBatchD>('b200z_inflate_batch');
   late final _InflateBatchDeviceD inflateBatchDevice =

@@ -108,6 +108,31 @@ int b200z_zlib_encode(const uint8_t *in, size_t in_len, int level, int window_bi
 /* GZipEncoderWeb().encodeBytes -- _gzip_encoder_web.dart:17-100 (MTIME is "now" in the reference: a parameter here) */
 int b200z_gzip_encode(const uint8_t *in, size_t in_len, int level, uint32_t mtime, uint8_t *out, size_t out_cap,
                       size_t *out_len);
+/* n independent b200z_gzip_decode / b200z_zlib_decode calls in one.  Stream i reads in_base[in_off[i] .. +in_len[i]) and
+ * writes out_base[out_off[i] .. +out_cap[i]); rc[i], out_len[i] and the bytes in its slot (up to out_len[i]) are exactly
+ * what the single call gives for that stream alone with out_cap[i]: B200Z_OK, B200Z_E_DATA and B200Z_E_THROW with their
+ * partial output, B200Z_E_NOSPC with the same out_len (the slot's contents unspecified).  `verify` of the gzip batch takes
+ * the B200Z_GZIP_VERIFY / B200Z_GZIP_RAW bits, as b200z_gzip_decode.  Input ranges may overlap or repeat; n == 0 is OK.
+ * Returns B200Z_OK unless an argument is wrong (null arrays, wrapping ranges, overlapping output slots: B200Z_E_ARG and
+ * nothing is written) or the device fails.  All inputs of a device group go up in one copy; per round, the hinted runs and
+ * the next member / zlib stream of every stream are one inflate batch, so a batch of single-member files is one launch
+ * chain where one call per file keeps one CTA busy.                                                                  */
+int b200z_gzip_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                            uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc);
+int b200z_zlib_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                            int raw, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                            int32_t *rc);
+/* n independent b200z_gzip_encode / b200z_zlib_encode calls in one: rc[i], out_len[i] and the slot's bytes as the single
+ * call gives them (B200Z_E_NOSPC: out_len[i] = the size needed, b200z_deflate_bound + 18 always suffices; an input of
+ * 4 GiB or more: B200Z_E_ARG, the others are still encoded).  An invalid level or windowBits is B200Z_E_ARG for the
+ * whole call; otherwise the argument rules of b200z_gzip_decode_batch.  One deflate batch (b200z_deflate_batch) for all
+ * inputs; the Adler-32 of all zlib inputs is one launch.                                                            */
+int b200z_gzip_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int level,
+                            uint32_t mtime, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                            uint64_t *out_len, int32_t *rc);
+int b200z_zlib_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int level,
+                            int window_bits, int raw, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                            uint64_t *out_len, int32_t *rc);
 
 /* BZip2Decoder().decodeBytes(data, verify:) -- bzip2_decoder.dart:13-88.  Stops after the first end-of-stream
  * block; CRCs are compared only when verify; B200Z_E_DATA == decodeStream returning false (the blocks decoded

@@ -1,14 +1,20 @@
-"""The on-disk side of the codec path (SURVEY.md 8f4): the reference's lib/src/io/extract_archive_to_disk.dart, for what this
-package decodes.  `extract_file_to_disk` runs the GZip / BZip2 stage of a compressed tar file -> file through the library's
-file entry point (b200z_file_codec: the bytes never pass through the host language), and unpacks .zip archives whose members
-were all decompressed by one device batch.  The tar CONTAINER is outside the scope contract (SURVEY.md section 8 lists the
-codecs and the ZIP container): for .tar.gz / .tgz / .tar.bz2 / .tbz the decompressed .tar is what lands in `output_path`."""
+"""The on-disk side of the codec path (SURVEY.md 8f4): the reference's lib/src/io/extract_archive_to_disk.dart and
+lib/src/io/tar_file_encoder.dart, for what this package decodes and encodes.  `extract_file_to_disk` runs the GZip / BZip2 /
+XZ stage of a compressed tar file -> file through the library's file entry point (b200z_file_codec: the bytes never pass
+through the host language), and unpacks .zip archives whose members were all decompressed by one device batch.  For
+.tar.gz / .tgz / .tar.bz2 / .tbz / .tar.xz / .txz it stops at the decompressed .tar in `output_path`, where the reference
+goes on to untar it; `extract_archive_to_disk(TarDecoder().decode_bytes(...), out)` unpacks a tar archive.
+`TarFileEncoder` writes a .tar or, through the same file entry point on the device, a .tar.gz."""
 from __future__ import annotations
 
 import os
+import shutil
+import tempfile
+import time
 
-from .codecs import BZip2Decoder, GZipDecoder, XZDecoder
+from .codecs import BZip2Decoder, GZipDecoder, GZipEncoder, XZDecoder
 from .streams import InputFileStream, OutputFileStream
+from .tar import TarEncoder
 from .zip import Archive, ArchiveFile, ZipDecoder
 
 
@@ -113,6 +119,17 @@ def extract_file_to_disk(input_path: str, output_path: str, buffer_size: int | N
     raise ValueError(f"{input_path}: must end with {_EXTENSIONS}")
 
 
+def _sorted_listing(dir_path: str, follow_links: bool) -> list:
+    """Directory.listSync(recursive: true, followLinks:) as [(path, is_directory)], sorted by path (the reference takes
+    whatever order the file system gives)."""
+    listing = []
+    for root, dirs, files in os.walk(dir_path, followlinks=follow_links):
+        dirs.sort()
+        listing += [(os.path.join(root, d), True) for d in dirs] + [(os.path.join(root, f), False) for f in sorted(files)]
+    listing.sort(key=lambda x: x[0])
+    return listing
+
+
 class ZipFileEncoder:
     """ZipFileEncoder (lib/src/io/zip_file_encoder.dart:11-225): build a .zip on disk from files and directories.  The
     reference compresses every file as it is added (ZipEncoder.startEncode / add / endEncode); here the members are collected
@@ -156,11 +173,7 @@ class ZipFileEncoder:
     def add_directory(self, dir_path: str, include_dir_name: bool = True, level=None, follow_links: bool = True, filter=None):
         """addDirectorySync (:93-136).  filter(path, progress) -> "skip" | "cancel" | anything else."""
         dir_name = os.path.basename(os.path.normpath(dir_path))
-        listing = []
-        for root, dirs, files in os.walk(dir_path, followlinks=follow_links):
-            dirs.sort()
-            listing += [(os.path.join(root, d), True) for d in dirs] + [(os.path.join(root, f), False) for f in sorted(files)]
-        listing.sort(key=lambda x: x[0])
+        listing = _sorted_listing(dir_path, follow_links)
         for k, (p, is_dir) in enumerate(listing):
             if filter is not None:
                 op = filter(p, (k + 1) / len(listing))
@@ -196,3 +209,85 @@ class ZipFileEncoder:
         self.create(self._compose_zip_directory_path(dir_path, filename), level=level, modified=modified)
         self.add_directory(dir_path, include_dir_name=False, level=level, follow_links=follow_links, filter=filter)
         return self.close()
+
+
+class TarFileEncoder:
+    """TarFileEncoder (lib/src/io/tar_file_encoder.dart:12-108): build a .tar, or a .tar.gz, on disk from files and
+    directories.  Members go through TarEncoder into an OutputFileStream as they are added; file contents are copied from
+    an InputFileStream.  Directory listings are taken in sorted order (the reference takes whatever order
+    Directory.listSync returns)."""
+    STORE, GZIP = 0, 1  # (:17-18)
+
+    def __init__(self):
+        self.tar_path, self._output, self._encoder = None, None, None
+
+    def tar_directory(self, dir_path: str, compression: int = STORE, filename=None, follow_links: bool = True,
+                      level=None, filter=None):
+        """tarDirectory (:20-49): `filename` or '<dir>.tar' / '<dir>.tar.gz', members named '<dir name>/...'.  For GZIP
+        the tar is written to a temporary `temp.tar` first, then GZipEncoder().encode_stream(InputFileStream,
+        OutputFileStream, level: level ?? 6) compresses it file to file on the device (b200z_file_codec), and the
+        temporary file and its directory are deleted."""
+        tar_path = filename if filename is not None else f"{dir_path}.tar"
+        tgz_path = filename if filename is not None else f"{dir_path}.tar.gz"
+        temp_dir = None
+        if compression == self.GZIP:
+            temp_dir = tempfile.mkdtemp(prefix="dart_archive")
+            tar_path = os.path.join(temp_dir, "temp.tar")
+        try:
+            self.open(tar_path)
+            self.add_directory(dir_path, follow_links=follow_links, filter=filter)
+            self.close()
+            if compression == self.GZIP:
+                inp, out = InputFileStream(tar_path), OutputFileStream(tgz_path)
+                try:
+                    GZipEncoder().encode_stream(inp, out, level=6 if level is None else level)
+                finally:
+                    inp.close_sync()
+                    out.close_sync()
+        finally:
+            if temp_dir is not None:
+                shutil.rmtree(temp_dir, ignore_errors=True)
+
+    def create(self, tar_path: str):  # (:51-58)
+        self.tar_path = tar_path
+        self._output = OutputFileStream(tar_path)
+        self._encoder = TarEncoder()
+        self._encoder.start(self._output)
+
+    open = create
+
+    def add_directory(self, dir_path: str, follow_links: bool = True, include_dir_name: bool = True, filter=None):
+        """addDirectory (:60-92).  filter(path, progress) -> "skip" | "cancel" | anything else.  A directory entry is
+        named '<name>/' and, as in the reference, carries the time it was added, not the directory's mtime."""
+        dir_name = os.path.basename(os.path.normpath(dir_path))
+        listing = _sorted_listing(dir_path, follow_links)
+        for k, (p, is_dir) in enumerate(listing):
+            if filter is not None:
+                op = filter(p, (k + 1) / len(listing))
+                if op == "cancel":
+                    break
+                if op == "skip":
+                    continue
+            rel = os.path.relpath(p, dir_path).replace(os.sep, "/")
+            name = f"{dir_name}/{rel}" if include_dir_name else rel
+            if is_dir:
+                f = ArchiveFile(f"{name}/", 0, is_file=False)  # ArchiveFile.directory: lastModTime is "now"
+                f.mode, f.last_mod_time = os.stat(p).st_mode, int(time.time())
+                self._encoder.add(f)
+            else:
+                self.add_file(p, name)
+
+    def add_file(self, path: str, filename=None):
+        """addFile (:94-102): the content is streamed from the file; the mode is the whole st_mode."""
+        st = os.stat(path)
+        inp = InputFileStream(path)
+        try:
+            f = ArchiveFile(filename if filename is not None else os.path.basename(path), inp.length)
+            f.content, f.last_mod_time, f.mode = inp, int(st.st_mtime), st.st_mode
+            self._encoder.add(f)
+        finally:
+            inp.close_sync()
+
+    def close(self):  # (:104-107)
+        self._encoder.finish()
+        self._output.close_sync()

@@ -42,11 +42,12 @@ def _name(raw: bytes) -> str:
 
 
 class ArchiveFile:
-    """archive_file.dart:14-130 (the fields ZipDecoder fills)."""
+    """archive_file.dart:14-130 (the fields ZipDecoder and TarDecoder fill)."""
 
     def __init__(self, name: str, size: int, is_file: bool = True):
         self.name, self.size, self.is_file = name, size, is_file
         self.mode = 0o644
+        self.owner_id = self.group_id = 0
         self.crc32 = None
         self.last_mod_time = 0
         self.compression = None

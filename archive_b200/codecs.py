@@ -201,13 +201,14 @@ class BZip2Decoder:
         return _stream_result(rc)
 
 
-def bzip2_decode_batch(streams, verify: bool = False) -> list:
+def bzip2_decode_batch(streams, verify: bool = False, device=None) -> list:
     """BZip2Decoder().decodeBytes(stream, verify:) for every stream of `streams` in one b200z_bzip2_decode_batch call:
     a list of (rc, bytes) in the same order.  rc is what b200z_bzip2_decode gives for that stream alone: OK, E_DATA
     (decodeStream returned false; bytes = the blocks decoded before the failure) or E_THROW (the reference throws a
     RangeError).  Each output room starts at BZip2Decoder's first guess; only the streams that did not fit are decoded
-    again, in larger rooms."""
+    again, in larger rooms.  device: see gzip_decode_batch."""
     L = _ffi.ensure_init()
+    sink = _Sink(device)
     views = [memoryview(s).cast("B") for s in streams]
     n = len(views)
     if n == 0:
@@ -233,12 +234,12 @@ def bzip2_decode_batch(streams, verify: bool = False) -> list:
         total = 0
         for k in range(m):
             a_out_off[k] = total
-            total += a_cap[k]
-        out = (C.c_uint8 * max(total, 1))()
+            total += sink.room(a_cap[k])
+        out, out_addr = sink.alloc(total)
         a_len = (C.c_uint64 * m)()
         a_rc = (C.c_int32 * m)()
-        _ffi.check(L.b200z_bzip2_decode_batch(C.addressof(in_buf), a_in_off, a_in_len, m, int(verify), C.addressof(out), a_out_off,
-                                              a_cap, a_len, a_rc))
+        _ffi.check(sink.call(L, "b200z_bzip2_decode_batch", C.addressof(in_buf), a_in_off, a_in_len, m, int(verify), out_addr,
+                             a_out_off, a_cap, a_len, a_rc))
         again = []
         for k, i in enumerate(todo):
             rc, got = a_rc[k], a_len[k]
@@ -248,7 +249,7 @@ def bzip2_decode_batch(streams, verify: bool = False) -> list:
                 continue
             if rc not in (_ffi.OK, _ffi.E_DATA, _ffi.E_THROW):
                 _ffi.check(rc)
-            result[i] = (rc, C.string_at(C.addressof(out) + a_out_off[k], got))
+            result[i] = (rc, sink.take(out, a_out_off[k], got))
         todo = again
     return result
 
@@ -349,6 +350,61 @@ def get_crc64(data) -> int:
     return crc.value
 
 
+class _Sink:
+    """Where a decode batch puts its output: host memory (device None: ctypes buffers, results as bytes), or one torch
+    CUDA buffer per call on the library's device (results as uint8 views, through the *_to_device entry points)."""
+
+    def __init__(self, device):
+        self.torch = None
+        if device is None:
+            return
+        import torch
+        dev = torch.device(device)
+        if dev.type == "cuda" and dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        _ffi.ensure_init()
+        if dev.type != "cuda" or dev.index != _ffi._inited_device:
+            raise ValueError(f"device {device!r} is not the library's CUDA device (cuda:{_ffi._inited_device})")
+        self.torch, self.device = torch, dev
+        # the caller's current stream; the legacy default stream (handle 0) is passed as cudaStreamLegacy (0x1), because
+        # NULL names the library's own stream
+        self.stream = torch.cuda.current_stream(dev).cuda_stream or 1
+
+    def room(self, cap):
+        """Bytes a slot of `cap` takes in the buffer: device slots start at 16-byte boundaries."""
+        return cap if self.torch is None else (cap + 15) & ~15
+
+    def alloc(self, total):
+        """(buffer, its address) for `total` bytes of slots."""
+        if self.torch is None:
+            buf = (C.c_uint8 * max(total, 1))()
+            return buf, C.addressof(buf)
+        buf = self.torch.empty(max(total, 1), dtype=self.torch.uint8, device=self.device)
+        return buf, buf.data_ptr()
+
+    def slots(self, sizes):
+        """(buffer, address, out_off, cap) for slots of `sizes` bytes, back to back."""
+        n = len(sizes)
+        out_off = (C.c_uint64 * n)()
+        cap = (C.c_uint64 * n)(*sizes)
+        total = 0
+        for i in range(n):
+            out_off[i] = total
+            total += self.room(sizes[i])
+        buf, addr = self.alloc(total)
+        return buf, addr, out_off, cap
+
+    def call(self, L, name, *args):
+        if self.torch is None:
+            return getattr(L, name)(*args)
+        return getattr(L, name + "_to_device")(*args, self.stream)
+
+    def take(self, buf, off, n):
+        if self.torch is None:
+            return C.string_at(C.addressof(buf) + off, n)
+        return buf[off:off + n]
+
+
 def _pack(items):
     """bytes-likes -> (ctypes buffer holding them back to back, in_off array, in_len array)."""
     views = [memoryview(s).cast("B") for s in items]
@@ -376,26 +432,28 @@ def _slots(sizes):
     return (C.c_uint8 * max(total, 1))(), out_off, cap
 
 
-def xz_decode_batch(streams, verify: bool = False) -> list:
+def xz_decode_batch(streams, verify: bool = False, device=None) -> list:
     """XZDecoder().decodeBytes(stream, verify:) for every stream of `streams` in one b200z_xz_decode_batch call: a list of
     (rc, bytes) in the same order.  rc is what b200z_xz_decode gives for that stream alone: OK, E_DATA (decodeStream
     returned false; bytes = what was written before it) or E_THROW (the reference throws a RangeError; bytes = the output
-    before the chunk that throws).  Each output room is b200z_xz_bound of its stream, which always suffices."""
+    before the chunk that throws).  Each output room is b200z_xz_bound of its stream, which always suffices.
+    device: see gzip_decode_batch."""
     L = _ffi.ensure_init()
+    sink = _Sink(device)
     n = len(streams)
     if n == 0:
         return []
     in_buf, in_off, in_len = _pack(streams)
     base = C.addressof(in_buf)
-    out, out_off, cap = _slots([L.b200z_xz_bound(base + in_off[i], in_len[i]) for i in range(n)])
+    out, out_addr, out_off, cap = sink.slots([L.b200z_xz_bound(base + in_off[i], in_len[i]) for i in range(n)])
     out_len = (C.c_uint64 * n)()
     rc = (C.c_int32 * n)()
-    _ffi.check(L.b200z_xz_decode_batch(base, in_off, in_len, n, int(verify), C.addressof(out), out_off, cap, out_len, rc))
+    _ffi.check(sink.call(L, "b200z_xz_decode_batch", base, in_off, in_len, n, int(verify), out_addr, out_off, cap, out_len, rc))
     result = []
     for i in range(n):
         if rc[i] not in (_ffi.OK, _ffi.E_DATA, _ffi.E_THROW):
             _ffi.check(rc[i])
-        result.append((rc[i], C.string_at(C.addressof(out) + out_off[i], out_len[i])))
+        result.append((rc[i], sink.take(out, out_off[i], out_len[i])))
     return result
 
 
@@ -420,10 +478,12 @@ def xz_encode_batch(contents, check: int = XZCheck.crc64) -> list:
 
 
 
-def _framed_decode_batch(call, streams, first_room) -> list:
+def _framed_decode_batch(call, streams, first_room, device) -> list:
     """One gzip / zlib decode batch over `streams` -> [(rc, bytes)]; only the streams that got E_NOSPC are decoded
-    again, in larger rooms (bzip2_decode_batch's rule)."""
+    again, in larger rooms (bzip2_decode_batch's rule).  call(L, sink, base, in_off, in_len, n, out, out_off, cap,
+    out_len, rc) makes the call through sink.call."""
     L = _ffi.ensure_init()
+    sink = _Sink(device)
     n = len(streams)
     if n == 0:
         return []
@@ -436,10 +496,10 @@ def _framed_decode_batch(call, streams, first_room) -> list:
         m = len(todo)
         a_in_off = (C.c_uint64 * m)(*[in_off[i] for i in todo])
         a_in_len = (C.c_uint64 * m)(*[in_len[i] for i in todo])
-        out, out_off, cap = _slots([rooms[i] for i in todo])
+        out, out_addr, out_off, cap = sink.slots([rooms[i] for i in todo])
         out_len = (C.c_uint64 * m)()
         rc = (C.c_int32 * m)()
-        _ffi.check(call(L, base, a_in_off, a_in_len, m, C.addressof(out), out_off, cap, out_len, rc))
+        _ffi.check(call(L, sink, base, a_in_off, a_in_len, m, out_addr, out_off, cap, out_len, rc))
         again = []
         for k, i in enumerate(todo):
             if rc[k] == _ffi.E_NOSPC and rooms[i] < (1 << 40):
@@ -448,27 +508,35 @@ def _framed_decode_batch(call, streams, first_room) -> list:
                 continue
             if rc[k] not in (_ffi.OK, _ffi.E_DATA, _ffi.E_THROW):
                 _ffi.check(rc[k])
-            result[i] = (rc[k], C.string_at(C.addressof(out) + out_off[k], out_len[k]))
+            result[i] = (rc[k], sink.take(out, out_off[k], out_len[k]))
         todo = again
     return result
 
 
-def gzip_decode_batch(streams, verify: bool = False, raw: bool = False) -> list:
+def gzip_decode_batch(streams, verify: bool = False, raw: bool = False, device=None) -> list:
     """GZipDecoder().decodeBytes(stream, verify:, raw:) for every stream of `streams` in one b200z_gzip_decode_batch call:
     a list of (rc, bytes) in the same order.  rc is what b200z_gzip_decode gives for that stream alone: OK, E_DATA
     (decodeStream returned false) or E_THROW (the reference throws a RangeError), with the bytes written before it.
-    Rooms start at b200z_gzip_bound (4n + 1024 when that is unknown)."""
+    Rooms start at b200z_gzip_bound (4n + 1024 when that is unknown).
+
+    device: None gives bytes.  A torch CUDA device (the library's) gives [(rc, tensor)] instead: each tensor is a 1-D
+    torch.uint8 view of the stream's out_len decoded bytes, inside one CUDA buffer per call (streams decoded again in
+    larger rooms get views of that call's buffer).  The decode goes straight into device memory
+    (b200z_*_decode_batch_to_device), ordered after the work already on torch.cuda.current_stream(); the tensors are
+    ready when the call returns."""
     flags = int(bool(verify)) | (2 if raw else 0)  # B200Z_GZIP_VERIFY | B200Z_GZIP_RAW
-    return _framed_decode_batch(lambda L, b, io, il, m, o, oo, cap, ol, rc: L.b200z_gzip_decode_batch(b, io, il, m, flags, o, oo, cap, ol, rc),
-                                streams, lambda L, a, n: L.b200z_gzip_bound(a, n) or 4 * n + 1024)
+    return _framed_decode_batch(lambda L, sink, b, io, il, m, o, oo, cap, ol, rc:
+                                sink.call(L, "b200z_gzip_decode_batch", b, io, il, m, flags, o, oo, cap, ol, rc),
+                                streams, lambda L, a, n: L.b200z_gzip_bound(a, n) or 4 * n + 1024, device)
 
 
-def zlib_decode_batch(streams, verify: bool = False, raw: bool = False) -> list:
+def zlib_decode_batch(streams, verify: bool = False, raw: bool = False, device=None) -> list:
     """ZLibDecoder().decodeBytes(stream, verify:, raw:) for every stream of `streams` in one b200z_zlib_decode_batch call:
-    a list of (rc, bytes) as gzip_decode_batch gives them, each what b200z_zlib_decode gives for that stream alone."""
-    return _framed_decode_batch(lambda L, b, io, il, m, o, oo, cap, ol, rc: L.b200z_zlib_decode_batch(b, io, il, m, int(verify), int(raw),
-                                                                                                     o, oo, cap, ol, rc),
-                                streams, lambda L, a, n: 4 * n + 1024)
+    a list of (rc, bytes) as gzip_decode_batch gives them, each what b200z_zlib_decode gives for that stream alone.
+    device: see gzip_decode_batch."""
+    return _framed_decode_batch(lambda L, sink, b, io, il, m, o, oo, cap, ol, rc:
+                                sink.call(L, "b200z_zlib_decode_batch", b, io, il, m, int(verify), int(raw), o, oo, cap, ol, rc),
+                                streams, lambda L, a, n: 4 * n + 1024, device)
 
 
 def _framed_encode_batch(call, contents) -> list:

@@ -22,7 +22,9 @@
 #include "bzip2_enc.h"
 #ifdef B200Z_EMU
 // The CPU emulation build of the library compiles the generated copies of the .cu files it lists; the encrypted-member
-// and XZ kernels come in here (zip_crypt_kernels.cu and xz_kernels.cu launch through macros both compilers take).
+// and XZ kernels come in here (zip_crypt_kernels.cu and xz_kernels.cu launch through macros both compilers take).  The
+// emulated runtime's pointer attributes come from the test tree (tests/host_emul/cuda_emu_pointer.h).
+#include "cuda_emu_pointer.h"
 #include "zip_crypt_kernels.cu"
 #include "xz_kernels.cu"
 #endif
@@ -116,6 +118,7 @@ struct Ctx {
   static const int kCompStreams = 8;
   cudaStream_t s_comp[kCompStreams] = {};
   DevBuf d_in, d_out, d_ws, d_meta, d_small, d_bz, d_tok, d_crypt;
+  DevBuf d_slots;  // the piece table of k_copy_slots (copy_slots)
   PinBuf h_meta, h_stage;  // h_stage: the outputs of a gzip / zlib decode batch on their way to the caller's slots (GZ_STAGE)
 };
 static Ctx g;
@@ -218,6 +221,97 @@ static int device_adler32_many(const uint8_t *base, const uint64_t *off, const u
 static int device_adler32(const uint8_t *d, size_t n, uint32_t *out) {
   const uint64_t off = 0, len = n;
   return device_adler32_many(d, &off, &len, 1, out);
+}
+
+// ---------------------------------------------------------------------------------------------
+// k_copy_slots: the device sink of the decode batches.  The host cuts every SlotCopy into pieces of at most COPY_PIECE bytes
+// and each warp takes one piece at a time, so a large slot spreads over many CTAs and small slots share one.  Stores are
+// 16-byte vectors from the destination's first 16-byte boundary on, with byte heads and tails.  When source and destination
+// disagree modulo 16, each stored vector is cut from the two aligned source vectors it straddles (both hold bytes of the
+// piece, so nothing outside the source's aligned 16-byte blocks is read).  Nothing outside [dst, dst + len) is written.
+// ---------------------------------------------------------------------------------------------
+constexpr uint64_t COPY_PIECE = 64u << 10;
+constexpr unsigned COPY_THREADS = 256;
+
+// bytes [4q + r/8, +16) of the 32 bytes a || b (q in 0..3, r in {0, 8, 16, 24}); q is the same for the whole warp
+__device__ __forceinline__ uint4 copy_shift16(const uint4 a, const uint4 b, uint32_t q, uint32_t r) {
+  switch (q) {
+    case 0: return make_uint4(__funnelshift_r(a.x, a.y, r), __funnelshift_r(a.y, a.z, r), __funnelshift_r(a.z, a.w, r), __funnelshift_r(a.w, b.x, r));
+    case 1: return make_uint4(__funnelshift_r(a.y, a.z, r), __funnelshift_r(a.z, a.w, r), __funnelshift_r(a.w, b.x, r), __funnelshift_r(b.x, b.y, r));
+    case 2: return make_uint4(__funnelshift_r(a.z, a.w, r), __funnelshift_r(a.w, b.x, r), __funnelshift_r(b.x, b.y, r), __funnelshift_r(b.y, b.z, r));
+    default: return make_uint4(__funnelshift_r(a.w, b.x, r), __funnelshift_r(b.x, b.y, r), __funnelshift_r(b.y, b.z, r), __funnelshift_r(b.z, b.w, r));
+  }
+}
+
+__global__ void __launch_bounds__(COPY_THREADS) k_copy_slots(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst,
+                                                            const SlotCopy *__restrict__ pieces, uint32_t n) {
+  const uint32_t lane = threadIdx.x & 31, n_warps = gridDim.x * (COPY_THREADS / 32);
+  for (uint32_t w = blockIdx.x * (COPY_THREADS / 32) + (threadIdx.x >> 5); w < n; w += n_warps) {
+    const SlotCopy c = pieces[w];
+    const uint8_t *s = src + c.src;
+    uint8_t *d = dst + c.dst;
+    const uint32_t to16 = (uint32_t)(-(uintptr_t)d & 15);
+    const uint32_t head = c.len < to16 ? (uint32_t)c.len : to16;
+    if (lane < head) d[lane] = s[lane];
+    const uint64_t nv = (c.len - head) >> 4;
+    uint4 *dv = (uint4 *)(d + head);
+    const uint8_t *sh = s + head;
+    const uint32_t k = (uint32_t)((uintptr_t)sh & 15);
+    const uint4 *sv = (const uint4 *)(sh - k);
+    if (k == 0) {
+      for (uint64_t i = lane; i < nv; i += 32) dv[i] = sv[i];
+    } else {
+      for (uint64_t i = lane; i < nv; i += 32) dv[i] = copy_shift16(sv[i], sv[i + 1], k >> 2, 8 * (k & 3));
+    }
+    for (uint64_t i = head + (nv << 4) + lane; i < c.len; i += 32) d[i] = s[i];
+  }
+}
+
+cudaError_t copy_slots(const uint8_t *src, uint8_t *dst, const SlotCopy *copies, size_t n, cudaStream_t s) {
+  std::vector<SlotCopy> pieces;
+  for (size_t i = 0; i < n; ++i)
+    for (uint64_t at = 0; at < copies[i].len; at += COPY_PIECE)
+      pieces.push_back(SlotCopy{copies[i].src + at, copies[i].dst + at, std::min(COPY_PIECE, copies[i].len - at)});
+  if (pieces.empty()) return cudaSuccess;
+  cudaError_t e = g.d_slots.reserve(pieces.size() * sizeof(SlotCopy));
+  if (e == cudaSuccess) e = cudaMemcpyAsync(g.d_slots.p, pieces.data(), pieces.size() * sizeof(SlotCopy), cudaMemcpyHostToDevice, s);
+  if (e != cudaSuccess) return e;
+  const size_t per_cta = COPY_THREADS / 32;
+  const unsigned grid = (unsigned)std::min<size_t>((pieces.size() + per_cta - 1) / per_cta, 1u << 16);
+  k_copy_slots<<<grid, COPY_THREADS, 0, s>>>(src, dst, (const SlotCopy *)g.d_slots.p, (uint32_t)pieces.size());
+  count_launch();
+  return cudaGetLastError();
+}
+
+// A *_to_device decode batch: d_out_base is device memory of the library's device whenever a slot has room (with no room
+// at all nothing is ever written, and the host batches' rules already let such a base be anything)
+static int device_out_arg(const char *name, const uint8_t *d_out_base, size_t n, const uint64_t *out_cap) {
+  bool room = false;
+  for (size_t i = 0; i < n && !room; ++i) room = out_cap[i] != 0;
+  if (!room) return B200Z_OK;
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, d_out_base) != cudaSuccess) {
+    cudaGetLastError();
+    set_err("%s: d_out_base is not a CUDA pointer", name);
+    return B200Z_E_ARG;
+  }
+  if (a.type != cudaMemoryTypeDevice || a.device != g.device) {
+    set_err("%s: d_out_base is not device memory of device %d", name, g.device);
+    return B200Z_E_ARG;
+  }
+  return B200Z_OK;
+}
+
+// the library's stream waits for what the caller enqueued on cuda_stream before the call (NULL: the library's own stream)
+static int wait_for_caller(void *cuda_stream) {
+  if (!cuda_stream) return B200Z_OK;
+  cudaEvent_t ev;
+  CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  const cudaError_t e1 = cudaEventRecord(ev, (cudaStream_t)cuda_stream);
+  const cudaError_t e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(g.stream, ev, 0) : e1;
+  cudaEventDestroy(ev);  // (released once it has completed)
+  CU(e2);
+  return B200Z_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1690,10 +1784,11 @@ static int gz_decode_group(std::vector<GzStream> &st, size_t a, size_t b, size_t
 }
 
 // n streams (arguments checked): rc[i] / out_len[i] / the slot's bytes as b200z_gzip_decode (gzip) or b200z_zlib_decode
-// give for stream i alone; `verify` takes B200Z_GZIP_VERIFY / B200Z_GZIP_RAW for gzip, a bool for zlib
+// give for stream i alone; `verify` takes B200Z_GZIP_VERIFY / B200Z_GZIP_RAW for gzip, a bool for zlib.  dev_out: out_base
+// is device memory on the library's device
 static int gzip_zlib_decode_streams(bool gzip, const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
                                     int verify, int raw, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap,
-                                    uint64_t *out_len, int32_t *rc) {
+                                    uint64_t *out_len, int32_t *rc, bool dev_out = false) {
   for (auto &v : g_gzb_stats) v = 0;
   g_gzb_stats[0] = n;
   std::vector<GzStream> st(n);
@@ -1740,35 +1835,45 @@ static int gzip_zlib_decode_streams(bool gzip, const uint8_t *in_base, const uin
       if (st[i].len) memcpy(packed.data() + st[i].din, st[i].h, st[i].len);
     int r = gz_decode_group(st, a, b, in_bytes, out_bytes, packed);
     if (r) return r;
-    // results, and the bytes of every stream that did not run out of room (the single calls copy nothing then).  The
-    // bytes come back through a pinned staging buffer of at most GZ_STAGE bytes, one asynchronous copy per stream and one
-    // synchronise per fill; a stream larger than the buffer is copied straight into its slot.
-    size_t i0 = a, o = 0;
-    auto drain = [&](size_t i1) -> int {  // streams [i0, i1) are in the staging buffer, back to back
+    if (dev_out) {  // device slots: the bytes of every stream that did not run out of room, in one k_copy_slots launch
+      std::vector<SlotCopy> cp;
+      for (size_t i = a; i < b; ++i) {
+        const size_t k = st[i].rc == B200Z_E_NOSPC ? 0 : std::min(st[i].out_len, st[i].cap);
+        if (k) cp.push_back(SlotCopy{st[i].dout, out_off[i], k});
+      }
+      CU(copy_slots((const uint8_t *)g.d_out.p, out_base, cp.data(), cp.size(), g.stream));
       CU(cudaStreamSynchronize(g.stream));
-      for (size_t p = 0; i0 < i1; ++i0) {
-        const size_t k = st[i0].rc == B200Z_E_NOSPC ? 0 : std::min(st[i0].out_len, st[i0].cap);
-        if (k && k <= GZ_STAGE) {
-          memcpy(out_base + out_off[i0], (const uint8_t *)g.h_stage.p + p, k);
-          p += k;
+    } else {
+      // results, and the bytes of every stream that did not run out of room (the single calls copy nothing then).  The
+      // bytes come back through a pinned staging buffer of at most GZ_STAGE bytes, one asynchronous copy per stream and one
+      // synchronise per fill; a stream larger than the buffer is copied straight into its slot.
+      size_t i0 = a, o = 0;
+      auto drain = [&](size_t i1) -> int {  // streams [i0, i1) are in the staging buffer, back to back
+        CU(cudaStreamSynchronize(g.stream));
+        for (size_t p = 0; i0 < i1; ++i0) {
+          const size_t k = st[i0].rc == B200Z_E_NOSPC ? 0 : std::min(st[i0].out_len, st[i0].cap);
+          if (k && k <= GZ_STAGE) {
+            memcpy(out_base + out_off[i0], (const uint8_t *)g.h_stage.p + p, k);
+            p += k;
+          }
+        }
+        o = 0;
+        return B200Z_OK;
+      };
+      for (size_t i = a; i < b; ++i) {
+        const size_t k = st[i].rc == B200Z_E_NOSPC ? 0 : std::min(st[i].out_len, st[i].cap);
+        const uint8_t *src = (const uint8_t *)g.d_out.p + st[i].dout;
+        if (k > GZ_STAGE) {
+          CU(cudaMemcpyAsync(out_base + out_off[i], src, k, cudaMemcpyDeviceToHost, g.stream));
+        } else if (k) {
+          if (o + k > GZ_STAGE && (r = drain(i)) != B200Z_OK) return r;
+          CU(g.h_stage.reserve(GZ_STAGE));
+          CU(cudaMemcpyAsync((uint8_t *)g.h_stage.p + o, src, k, cudaMemcpyDeviceToHost, g.stream));
+          o += k;
         }
       }
-      o = 0;
-      return B200Z_OK;
-    };
-    for (size_t i = a; i < b; ++i) {
-      const size_t k = st[i].rc == B200Z_E_NOSPC ? 0 : std::min(st[i].out_len, st[i].cap);
-      const uint8_t *src = (const uint8_t *)g.d_out.p + st[i].dout;
-      if (k > GZ_STAGE) {
-        CU(cudaMemcpyAsync(out_base + out_off[i], src, k, cudaMemcpyDeviceToHost, g.stream));
-      } else if (k) {
-        if (o + k > GZ_STAGE && (r = drain(i)) != B200Z_OK) return r;
-        CU(g.h_stage.reserve(GZ_STAGE));
-        CU(cudaMemcpyAsync((uint8_t *)g.h_stage.p + o, src, k, cudaMemcpyDeviceToHost, g.stream));
-        o += k;
-      }
+      if ((r = drain(b)) != B200Z_OK) return r;
     }
-    if ((r = drain(b)) != B200Z_OK) return r;
     for (size_t i = a; i < b; ++i) {
       out_len[i] = st[i].out_len;
       rc[i] = st[i].rc;
@@ -1891,8 +1996,10 @@ static inline uint32_t be32_in_tail(const uint8_t *tail8, uint64_t len, uint64_t
 // BZip2Decoder.decodeStream for n streams whose bytes are on the device already.  K6 scans all of them in one launch; the
 // streams are then cut into consecutive device groups that fit the memory budget, and each group takes one K7 and one K8
 // over the blocks of all its streams, each stream's output going to a slot of its own.  Returns B200Z_OK unless the device
-// fails; each stream's result is in its job.
-static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, int verify, Bz2Shard *shard = nullptr) {
+// fails; each stream's result is in its job.  dev_out != nullptr: the jobs' slots are device memory from dev_out on, and each
+// delivery is one k_copy_slots launch for the streams it serves instead of one copy to the host per stream.
+static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, int verify, Bz2Shard *shard = nullptr,
+                               uint8_t *dev_out = nullptr) {
   g_bz2_stats[0] = n;
   g_bz2_stats[1] = g_bz2_stats[2] = 0;
   if (n == 0) return B200Z_OK;
@@ -2210,17 +2317,22 @@ static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, in
     std::vector<int32_t> h_irr(nc);
     // the bytes of the chain entries below `hi` are written: those in the streams' slots go to the host on the copy stream
     auto copy_early = [&](uint32_t hi) -> int {
+      std::vector<SlotCopy> cp;
       for (size_t q = 0; q < G; ++q) {
         if (ch_lo[q] >= hi || ch_lo[q] == ch_lo[q + 1]) continue;
         const uint32_t last = std::min(hi, ch_lo[q + 1]) - 1;
         const unsigned long long end = std::min(h_off[last] + h_out[last], s_hi[q]);
         if (end > early[q]) {
-          CU(cudaMemcpyAsync(jobs[grp[q]].out + (early[q] - s_lo[q]), (uint8_t *)g.d_out.p + early[q], end - early[q],
-                             cudaMemcpyDeviceToHost, g.s_d2h));
+          if (dev_out)
+            cp.push_back(SlotCopy{early[q], (uint64_t)(jobs[grp[q]].out - dev_out) + (early[q] - s_lo[q]), end - early[q]});
+          else
+            CU(cudaMemcpyAsync(jobs[grp[q]].out + (early[q] - s_lo[q]), (uint8_t *)g.d_out.p + early[q], end - early[q],
+                               cudaMemcpyDeviceToHost, g.s_d2h));
           early[q] = end;
           any_early = true;
         }
       }
+      if (dev_out) CU(copy_slots((const uint8_t *)g.d_out.p, dev_out, cp.data(), cp.size(), g.s_d2h));
       return B200Z_OK;
     };
     if (nc) {
@@ -2285,8 +2397,12 @@ static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, in
           cudaEventDestroy(ev[gi]);
           const unsigned long long end = std::min((unsigned long long)h_end_off[gi], s_hi[0]);
           if (end > early[0]) {
-            CU(cudaMemcpyAsync(jobs[grp[0]].out + early[0], (uint8_t *)g.d_out.p + early[0], end - early[0], cudaMemcpyDeviceToHost,
-                               g.s_d2h));
+            const SlotCopy c{early[0], dev_out ? (uint64_t)(jobs[grp[0]].out - dev_out) + early[0] : 0, end - early[0]};
+            if (dev_out)
+              CU(copy_slots((const uint8_t *)g.d_out.p, dev_out, &c, 1, g.s_d2h));
+            else
+              CU(cudaMemcpyAsync(jobs[grp[0]].out + early[0], (uint8_t *)g.d_out.p + early[0], end - early[0], cudaMemcpyDeviceToHost,
+                                 g.s_d2h));
             early[0] = end;
             any_early = true;
           }
@@ -2349,6 +2465,7 @@ static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, in
     }
     // blocks are committed in order; the first bad one ends the stream (its bytes are already written when the
     // reference compares the CRC, :58-66)
+    std::vector<SlotCopy> cp;
     for (size_t q = 0; q < G; ++q) {
       Bz2Job &j = jobs[grp[q]];
       int final_rc = s_rc[q];
@@ -2389,9 +2506,12 @@ static int bzip2_decode_device(const uint8_t *d_base, Bz2Job *jobs, size_t n, in
       }
       j.rc = final_rc;
       const size_t from = (size_t)(early[q] - s_lo[q]);
-      if (n_out > from)
+      if (n_out > from && dev_out)
+        cp.push_back(SlotCopy{s_lo[q] + from, (uint64_t)(j.out - dev_out) + from, n_out - from});
+      else if (n_out > from)
         CU(cudaMemcpyAsync(j.out + from, (uint8_t *)g.d_out.p + s_lo[q] + from, n_out - from, cudaMemcpyDeviceToHost, g.stream));
     }
+    if (dev_out) CU(copy_slots((const uint8_t *)g.d_out.p, dev_out, cp.data(), cp.size(), g.stream));
     CU(cudaStreamSynchronize(g.stream));
   }
   return B200Z_OK;
@@ -3837,8 +3957,11 @@ int b200z_bzip2_decode(const uint8_t *in, size_t in_len, int verify, uint8_t *ou
   return rc ? rc : j.rc;
 }
 
-int b200z_bzip2_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
-                             uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+}  // extern "C"
+// b200z_bzip2_decode_batch, or b200z_bzip2_decode_batch_to_device with a stream (dev_out)
+static int bzip2_decode_batch_impl(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                   uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                                   int32_t *rc, bool dev_out, void *cuda_stream) {
   int r = require_init();
   if (r) return r;
   if (n && (!in_off || !in_len || !out_off || !out_cap || !out_len || !rc)) {
@@ -3866,9 +3989,11 @@ int b200z_bzip2_decode_batch(const uint8_t *in_base, const uint64_t *in_off, con
       set_err("bzip2_decode_batch: output slots %zu and %zu overlap", by_out[k - 1], by_out[k]);
       return B200Z_E_ARG;
     }
+  if (dev_out && (r = device_out_arg("bzip2_decode_batch_to_device", out_base, n, out_cap)) != B200Z_OK) return r;
   std::lock_guard<std::mutex> lk(g.mu);
   if (n == 0) return bzip2_decode_device(nullptr, nullptr, 0, verify);
   CU(cudaSetDevice(g.device));
+  if (dev_out && (r = wait_for_caller(cuda_stream)) != B200Z_OK) return r;
   // one copy to the device: the span of all inputs as it is, or the inputs packed when the span is mostly other bytes
   std::vector<Bz2Job> jobs(n);
   std::vector<uint8_t> packed;
@@ -3897,12 +4022,22 @@ int b200z_bzip2_decode_batch(const uint8_t *in_base, const uint64_t *in_off, con
     jobs[i].out = out_base + out_off[i];
     jobs[i].out_cap = out_cap[i];
   }
-  r = bzip2_decode_device((const uint8_t *)g.d_in.p, jobs.data(), n, verify);
+  r = bzip2_decode_device((const uint8_t *)g.d_in.p, jobs.data(), n, verify, nullptr, dev_out ? out_base : nullptr);
   for (size_t i = 0; i < n; ++i) {
     out_len[i] = jobs[i].out_len;
     rc[i] = jobs[i].rc;
   }
   return r;
+}
+extern "C" {
+int b200z_bzip2_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                             uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
+  return bzip2_decode_batch_impl(in_base, in_off, in_len, n, verify, out_base, out_off, out_cap, out_len, rc, false, nullptr);
+}
+int b200z_bzip2_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                                       int verify, uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                       uint64_t *out_len, int32_t *rc, void *cuda_stream) {
+  return bzip2_decode_batch_impl(in_base, in_off, in_len, n, verify, d_out_base, out_off, out_cap, out_len, rc, true, cuda_stream);
 }
 // (test hooks, not part of the ABI) cap on the blocks of one BZip2 device group (0: the memory budget alone); the last
 // b200z_bzip2_decode* or ZIP call's bzip2 streams, device groups and blocks
@@ -3989,6 +4124,18 @@ int b200z_xz_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const 
   std::lock_guard<std::mutex> lk(g.mu);
   CU(cudaSetDevice(g.device));
   return xz_decode_streams(in_base, in_off, in_len, n, verify, out_base, out_off, out_cap, out_len, rc, g.stream);
+}
+int b200z_xz_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                    uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                                    int32_t *rc, void *cuda_stream) {
+  int r = require_init();
+  if (r) return r;
+  r = xz_batch_args("xz_decode_batch_to_device", in_base, in_off, in_len, n, d_out_base, out_off, out_cap, out_len, rc);
+  if (r || (r = device_out_arg("xz_decode_batch_to_device", d_out_base, n, out_cap))) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  if ((r = wait_for_caller(cuda_stream))) return r;
+  return xz_decode_streams(in_base, in_off, in_len, n, verify, d_out_base, out_off, out_cap, out_len, rc, g.stream, true);
 }
 int b200z_xz_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
                           uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc) {
@@ -4117,6 +4264,7 @@ void b200z_shutdown(void) {
   cudaSetDevice(g.device);
   cudaStreamSynchronize(g.stream);
   g.d_in.release(); g.d_out.release(); g.d_ws.release(); g.d_meta.release(); g.d_small.release(); g.d_bz.release(); g.d_tok.release(); g.d_crypt.release();
+  g.d_slots.release();
   g.h_meta.release(); g.h_stage.release();
   cudaStreamDestroy(g.stream);
   cudaStreamDestroy(g.s_h2d);
@@ -4402,6 +4550,30 @@ int b200z_zlib_decode_batch(const uint8_t *in_base, const uint64_t *in_off, cons
   std::lock_guard<std::mutex> lk(g.mu);
   CU(cudaSetDevice(g.device));
   return gzip_zlib_decode_streams(false, in_base, in_off, in_len, n, verify, raw, out_base, out_off, out_cap, out_len, rc);
+}
+int b200z_gzip_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                      uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                                      int32_t *rc, void *cuda_stream) {
+  int r = require_init();
+  if (r) return r;
+  r = xz_batch_args("gzip_decode_batch_to_device", in_base, in_off, in_len, n, d_out_base, out_off, out_cap, out_len, rc);
+  if (r || (r = device_out_arg("gzip_decode_batch_to_device", d_out_base, n, out_cap))) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  if ((r = wait_for_caller(cuda_stream))) return r;
+  return gzip_zlib_decode_streams(true, in_base, in_off, in_len, n, verify, 0, d_out_base, out_off, out_cap, out_len, rc, true);
+}
+int b200z_zlib_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                      int raw, uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                      uint64_t *out_len, int32_t *rc, void *cuda_stream) {
+  int r = require_init();
+  if (r) return r;
+  r = xz_batch_args("zlib_decode_batch_to_device", in_base, in_off, in_len, n, d_out_base, out_off, out_cap, out_len, rc);
+  if (r || (r = device_out_arg("zlib_decode_batch_to_device", d_out_base, n, out_cap))) return r;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  if ((r = wait_for_caller(cuda_stream))) return r;
+  return gzip_zlib_decode_streams(false, in_base, in_off, in_len, n, verify, raw, d_out_base, out_off, out_cap, out_len, rc, true);
 }
 int b200z_gzip_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int level,
                             uint32_t mtime, uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,

@@ -146,6 +146,14 @@ size_t bz2_slot_bytes_per_block();
 cudaError_t bz2_launch_ibwt(const Bz2Ibwt &a, cudaStream_t s);
 cudaError_t bz2_launch_ibwt_group(const Bz2Ibwt &a, uint32_t lo, uint32_t hi, cudaStream_t s);
 void count_launch();
+// The device sink of the decode batches (b200z_*_decode_batch_to_device): one copy of `len` bytes from the library's group
+// buffer (src + src) into a slot of the caller's device buffer (dst + dst).
+struct SlotCopy {
+  uint64_t src, dst, len;
+};
+// every copy of `copies` as one k_copy_slots launch on stream s, not synchronised (nothing when there is no byte to copy);
+// the table goes up on s, so launches on one stream may follow each other freely
+cudaError_t copy_slots(const uint8_t *src, uint8_t *dst, const SlotCopy *copies, size_t n, cudaStream_t s);
 void profile_enable(bool on);
 int profile_read(double *fast_ms, double *decode_ms, double *expand_ms, uint64_t *n);
 
@@ -221,10 +229,11 @@ cudaError_t zip_launch_zipcrypto(const ZipCryptoMember *d_m, uint32_t n, const u
 // ---- XZ (xz_kernels.cu): host buffers in, host buffers out, blocking on `s` ----
 size_t xz_bound(const uint8_t *in, size_t n);  // the output the container declares, up to where its walk stops
 // n streams (arguments checked): rc[i] / out_len[i] / bytes as xz_decode_impl / xz_encode_impl give for stream i alone;
-// the return value is B200Z_OK, B200Z_E_ARG (encode: a bad check kind) or a device failure
+// the return value is B200Z_OK, B200Z_E_ARG (encode: a bad check kind) or a device failure.  dev_out: out_base is device
+// memory (the decode's bytes go to the slots through k_copy_slots, one launch per device group)
 int xz_decode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
-                      cudaStream_t s);
+                      cudaStream_t s, bool dev_out = false);
 int xz_encode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
                       cudaStream_t s);

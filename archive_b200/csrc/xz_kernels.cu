@@ -979,9 +979,11 @@ size_t xz_bound(const uint8_t *in, size_t n) {
 
 // Decode the planned streams jobs[0..m) as one device group: one copy up of the inputs and one of the tables, one
 // k_xz_copy, one k_xz_lzma over the runs of all streams, one CRC launch per check kind, one copy back of the chunk
-// statuses and tile CRCs.  Then each stream replays its own events, and its bytes go to its slot.
+// statuses and tile CRCs.  Then each stream replays its own events, and its bytes go to its slot: one copy per stream into
+// host slots, one k_copy_slots launch for the whole group into device slots (dev_out).
 static int xz_decode_group(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, XzJob *jobs, size_t m,
-                           uint8_t *out_base, const uint64_t *out_off, uint64_t *out_len, int32_t *rc, cudaStream_t s) {
+                           uint8_t *out_base, const uint64_t *out_off, uint64_t *out_len, int32_t *rc, cudaStream_t s,
+                           bool dev_out) {
   // ---- the group's tables: chunks, runs and check ranges rebased onto the staged input and the device output ----
   std::vector<size_t> idx(m);
   std::vector<uint64_t> in_dev;
@@ -1094,6 +1096,7 @@ static int xz_decode_group(const uint8_t *in_base, const uint64_t *in_off, const
   const int32_t *status = (const int32_t *)res.data();
   uint64_t got_all = 0;
   bool failed = false;
+  std::vector<SlotCopy> to_dev;
   for (size_t j = 0; j < m; ++j) {
     const XzJob &J = jobs[j];
     const XzPlan &p = J.p;
@@ -1126,13 +1129,16 @@ static int xz_decode_group(const uint8_t *in_base, const uint64_t *in_off, const
     }
     if (r == p.status && r == B200Z_E_DATA) set_error_text("xz_decode: the stream is not valid XZ (decodeStream returned false)");
     if (r == p.status && r == B200Z_E_THROW) set_error_text("xz_decode: the container walk reads past the input (Dart: RangeError)");
-    if (got)
+    if (got && dev_out)
+      to_dev.push_back(SlotCopy{J.out_dev, out_off[J.i], got});
+    else if (got)
       XZ_CU(cudaMemcpyAsync(out_base + out_off[J.i], (const uint8_t *)x_out.p + J.out_dev, (size_t)got, cudaMemcpyDeviceToHost, s));
     rc[J.i] = r;
     out_len[J.i] = got;
     got_all += got;
     failed |= r != B200Z_OK;
   }
+  if (dev_out) XZ_CU(copy_slots((const uint8_t *)x_out.p, out_base, to_dev.data(), to_dev.size(), s));
   XZ_CU(cudaStreamSynchronize(s));
   // a damaged stream can declare far more output than it yields (each 6-byte LZMA chunk header up to 2 MiB): the
   // reservation made for it is not kept for the life of the library
@@ -1142,7 +1148,7 @@ static int xz_decode_group(const uint8_t *in_base, const uint64_t *in_off, const
 
 int xz_decode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
-                      cudaStream_t s) {
+                      cudaStream_t s, bool dev_out) {
   g_xz_lzma_ms = 0;
   g_xz_runs = 0;
   g_xz_stats[0] = n;
@@ -1195,7 +1201,7 @@ int xz_decode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint
       lclp = l2;
     }
     g_xz_stats[1]++;
-    const int r = xz_decode_group(in_base, in_off, in_len, jobs.data() + k, e - k, out_base, out_off, out_len, rc, s);
+    const int r = xz_decode_group(in_base, in_off, in_len, jobs.data() + k, e - k, out_base, out_off, out_len, rc, s, dev_out);
     if (r) return r;
     k = e;
   }

@@ -50,6 +50,20 @@ typedef _ZlibDecodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64
 typedef _ZlibDecodeBatchD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
     int verify, int raw, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
     Pointer<Int32> rc);
+// b200z_{gzip,bzip2,xz}_decode_batch_to_device: the host batch's arguments, then the cudaStream_t (dOutBase is device memory)
+typedef _DecodeBatchToDeviceC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Int32 verify, Pointer<Uint8> dOutBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc, Pointer<Void> cudaStream);
+typedef _DecodeBatchToDeviceD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    int verify, Pointer<Uint8> dOutBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc, Pointer<Void> cudaStream);
+// b200z_zlib_decode_batch_to_device: (inBase, inOff, inLen, n, verify, raw, dOutBase, outOff, outCap, outLen, rc, cudaStream)
+typedef _ZlibDecodeBatchToDeviceC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
+    Int32 verify, Int32 raw, Pointer<Uint8> dOutBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc, Pointer<Void> cudaStream);
+typedef _ZlibDecodeBatchToDeviceD = int Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, int n,
+    int verify, int raw, Pointer<Uint8> dOutBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap, Pointer<Uint64> outLen,
+    Pointer<Int32> rc, Pointer<Void> cudaStream);
 // b200z_gzip_encode_batch: (inBase, inOff, inLen, n, level, mtime, outBase, outOff, outCap, outLen, rc)
 typedef _GzipEncodeBatchC = Int32 Function(Pointer<Uint8> inBase, Pointer<Uint64> inOff, Pointer<Uint64> inLen, Size n,
     Int32 level, Uint32 mtime, Pointer<Uint8> outBase, Pointer<Uint64> outOff, Pointer<Uint64> outCap,
@@ -297,6 +311,14 @@ class B200Z {
       _lib.lookupFunction<_Bz2DecodeBatchC, _Bz2DecodeBatchD>('b200z_gzip_decode_batch');
   late final _ZlibDecodeBatchD zlibDecodeBatch =
       _lib.lookupFunction<_ZlibDecodeBatchC, _ZlibDecodeBatchD>('b200z_zlib_decode_batch');
+  late final _DecodeBatchToDeviceD gzipDecodeBatchToDevice =
+      _lib.lookupFunction<_DecodeBatchToDeviceC, _DecodeBatchToDeviceD>('b200z_gzip_decode_batch_to_device');
+  late final _ZlibDecodeBatchToDeviceD zlibDecodeBatchToDevice =
+      _lib.lookupFunction<_ZlibDecodeBatchToDeviceC, _ZlibDecodeBatchToDeviceD>('b200z_zlib_decode_batch_to_device');
+  late final _DecodeBatchToDeviceD bzip2DecodeBatchToDevice =
+      _lib.lookupFunction<_DecodeBatchToDeviceC, _DecodeBatchToDeviceD>('b200z_bzip2_decode_batch_to_device');
+  late final _DecodeBatchToDeviceD xzDecodeBatchToDevice =
+      _lib.lookupFunction<_DecodeBatchToDeviceC, _DecodeBatchToDeviceD>('b200z_xz_decode_batch_to_device');
   late final _GzipEncodeBatchD gzipEncodeBatch =
       _lib.lookupFunction<_GzipEncodeBatchC, _GzipEncodeBatchD>('b200z_gzip_encode_batch');
   late final _ZlibEncodeBatchD zlibEncodeBatch =

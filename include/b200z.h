@@ -226,6 +226,36 @@ int b200z_xz_decode_batch(const uint8_t *in_base, const uint64_t *in_off, const 
 int b200z_xz_encode_batch(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
                           uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc);
 
+/* ---- decode batches into device memory ------------------------------------------------------------------------------
+ * b200z_gzip_decode_batch_to_device / _zlib_ / _bzip2_ / _xz_ = the host batch of the same name with the output slots in
+ * device memory, so that decoded bytes never make the round trip through the host.
+ *   Memory: the inputs and every array (in_off, in_len, out_off, out_cap, out_len, rc) are host memory, as in the host
+ *     batch (the framing rules read the compressed bytes on the host).  d_out_base is device memory on the b200z_init device.
+ *   Results: for every stream, rc[i], out_len[i] and the bytes in the slot d_out_base[out_off[i] .. +out_cap[i]) are exactly
+ *     what the host batch gives for the same arguments; after B200Z_E_NOSPC the slot's contents are unspecified.  Nothing is
+ *     written outside the slots; slots may come in any order, leave gaps and start at any byte alignment.
+ *   Argument errors: the host batch's rules (null arrays, wrapping ranges, overlapping slots), and d_out_base must be device
+ *     memory of the library's device (cudaPointerGetAttributes) whenever a slot has room: B200Z_E_ARG, nothing is written.
+ *     n == 0 is OK.  No device (b200z_init not called or failed): B200Z_E_NODEVICE.
+ *   Ordering: the library's stream waits on an event recorded on cuda_stream (a cudaStream_t; NULL = the library's own
+ *     stream, cudaStreamLegacy for the legacy default stream) when the call starts, so work enqueued there before the call
+ *     comes before any write to the slots.  The call returns once the bytes are in place, like the host batches: the output
+ *     may be used on any stream from then on.
+ * Each device group's results go from the library's buffer into the slots with one k_copy_slots launch (one per delivery
+ * point for BZip2), whatever the number of streams.                                                                     */
+int b200z_gzip_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                      uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                                      int32_t *rc, void *cuda_stream);
+int b200z_zlib_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                      int raw, uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                      uint64_t *out_len, int32_t *rc, void *cuda_stream);
+int b200z_bzip2_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n,
+                                       int verify, uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap,
+                                       uint64_t *out_len, int32_t *rc, void *cuda_stream);
+int b200z_xz_decode_batch_to_device(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
+                                    uint8_t *d_out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len,
+                                    int32_t *rc, void *cuda_stream);
+
 /* ---- ZIP container: ZipDecoder / ZipDirectory / ZipFileHeader / ZipFile ------------------------------------
  * b200z_zip_list   = ZipDirectory.read (zip_directory.dart:25-183) + ZipFileHeader.read (zip_file_header.dart:28-111)
  *                    + ZipFile.read (zip_file.dart:73-149), host only: no device is needed.

@@ -113,6 +113,10 @@ _SIGS = {
                                        C.POINTER(C.c_uint32)]),
     "b200z_zip_extract_password": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]),
+    # b200z_zip_extract_password with its slots in device memory, plus the member CRC-32s and the caller's cudaStream_t
+    "b200z_zip_extract_to_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                              C.c_size_t, C.c_void_p]),
     "b200z_zip_aes_encrypt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
                                         C.c_void_p, C.c_void_p]),
     "b200z_bzip2_decode_shard": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,

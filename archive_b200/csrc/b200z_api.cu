@@ -290,7 +290,7 @@ static int device_out_arg(const char *name, const uint8_t *d_out_base, size_t n,
   for (size_t i = 0; i < n && !room; ++i) room = out_cap[i] != 0;
   if (!room) return B200Z_OK;
   cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, d_out_base) != cudaSuccess) {
+  if (!d_out_base || cudaPointerGetAttributes(&a, d_out_base) != cudaSuccess) {
     cudaGetLastError();
     set_err("%s: d_out_base is not a CUDA pointer", name);
     return B200Z_E_ARG;
@@ -3199,11 +3199,15 @@ static int zip_chunked(const uint8_t *z, size_t len, const b200z_zip_entry *entr
   return B200Z_OK;
 }
 
+static uint64_t g_zip_out_bytes = 0;  // (test hook) g.d_out bytes the last ZIP extract asked for
+
 // ZipFile.getStream for all members (g.mu held).  pl == nullptr: the archive is not staged yet and `len` is its size;
-// otherwise `len` = pl->staged and everything is in g.d_in already.
+// otherwise `len` = pl->staged and everything is in g.d_in already.  Deflate, stored and K12 members decode into g.d_out,
+// which holds the slots' span [lo, hi) only (offset out_off[i] - lo); dev_out: `out` is device memory, and the bytes go
+// from g.d_out into the slots with one k_copy_slots launch instead of the copies of [lo, hi) to the host.
 static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                             size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
-                            int32_t *status, uint32_t flags, const ZipPlain *pl) {
+                            int32_t *status, uint32_t flags, const ZipPlain *pl, bool dev_out) {
   int rc = B200Z_OK;
   // members: deflate -> one inflate batch; stored (and unknown methods, which the reference treats as stored,
   // zip_file.dart:83) -> device copies; bzip2 -> one BZip2 batch, afterwards
@@ -3256,19 +3260,24 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
     }
   }
   const bool any_dev = hi > lo;
+  if (!any_dev) lo = hi = 0;
+  // units live at out_off - lo in g.d_out; a unit without room may name any offset, and keeps its order among the others
+  for (auto &o : u_out_off) o = std::min(std::max(o, lo), hi) - lo;
+  g_zip_out_bytes = 0;
   if (any_dev || !u_idx.empty() || !bz_idx.empty()) {
     if (!pl) {
       rc = stage_input(z, len);
       if (rc) return rc;
     }
     CU(cudaMemsetAsync((uint8_t *)g.d_in.p + len, 0, 64, g.stream));
-    CU(g.d_out.reserve((hi ? hi : 1) + 64));
+    g_zip_out_bytes = std::max<uint64_t>(hi - lo, 1) + 64;
+    CU(g.d_out.reserve(g_zip_out_bytes));
   }
   for (size_t i = 0; i < n; ++i) {
     const b200z_zip_entry &e = entries[i];
     if (!e.has_data || (e.flags & 1u) || e.method == 8 || e.method == 12) continue;
     uint64_t k = e.comp_size < out_room[i] ? e.comp_size : out_room[i];
-    if (k) CU(cudaMemcpyAsync((uint8_t *)g.d_out.p + out_off[i], (const uint8_t *)g.d_in.p + e.data_off, k, cudaMemcpyDeviceToDevice, g.stream));
+    if (k) CU(cudaMemcpyAsync((uint8_t *)g.d_out.p + (out_off[i] - lo), (const uint8_t *)g.d_in.p + e.data_off, k, cudaMemcpyDeviceToDevice, g.stream));
     out_len[i] = e.comp_size;
     if (e.comp_size > out_room[i]) status[i] = B200Z_U_NOSPC;
   }
@@ -3369,8 +3378,9 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
     std::vector<int32_t> r_st(m);
     // A large archive is decoded in chunks of units (in output order), and the bytes of a finished chunk -- with the stored
     // members that lie between its units -- go to the host on the copy stream while the next chunk is decoded
-    // (B200Z_ZIP_CHUNKS, default 8 from 512 MiB of output on; 1: one batch, one copy at the end).
-    size_t nchunks = (hi - lo) >= ((size_t)512 << 20) ? 8 : 1;
+    // (B200Z_ZIP_CHUNKS, default 8 from 512 MiB of output on; 1: one batch, one copy at the end).  Device slots have no
+    // PCIe copy to hide: one batch by default, and chunks (when asked for) deliver nothing early.
+    size_t nchunks = !dev_out && (hi - lo) >= ((size_t)512 << 20) ? 8 : 1;
     if (const char *ce = getenv("B200Z_ZIP_CHUNKS")) nchunks = (size_t)std::max(1, atoi(ce));
     for (size_t k = 1; k < m && nchunks > 1; ++k)
       if (u_out_off[k] < u_out_off[k - 1]) nchunks = 1;  // (units are made in output order; if ever not, no early copies)
@@ -3379,14 +3389,15 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
       const size_t k1 = m * (c + 1) / nchunks;
       if (k1 == k0) continue;
       rc = run_batch_on_staged(u_in_off.data() + k0, u_in_len.data() + k0, u_out_off.data() + k0, u_cap.data() + k0, r_len.data() + k0,
-                               r_st.data() + k0, r_used.data() + k0, k1 - k0, (size_t)hi);
+                               r_st.data() + k0, r_used.data() + k0, k1 - k0, (size_t)(hi - lo));
       if (rc) {
         if (early_to > lo) cudaStreamSynchronize(g.s_d2h);
         return rc;
       }
-      const size_t end = k1 < m ? (size_t)u_out_off[k1] : (size_t)hi;
-      if (nchunks > 1 && end > early_to && end <= hi) {
-        CU(cudaMemcpyAsync(out + early_to, (const uint8_t *)g.d_out.p + early_to, end - early_to, cudaMemcpyDeviceToHost, g.s_d2h));
+      const size_t end = k1 < m ? (size_t)(lo + u_out_off[k1]) : (size_t)hi;
+      if (nchunks > 1 && !dev_out && end > early_to && end <= hi) {
+        CU(cudaMemcpyAsync(out + early_to, (const uint8_t *)g.d_out.p + (early_to - lo), end - early_to, cudaMemcpyDeviceToHost,
+                           g.s_d2h));
         early_to = end;
       }
       k0 = k1;
@@ -3402,9 +3413,19 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
       }
     }
   }
-  if (any_dev) {
+  if (any_dev && dev_out) {  // each member's bytes into its slot, one k_copy_slots launch for all of them
+    std::vector<SlotCopy> cp;
+    for (size_t i = 0; i < n; ++i) {
+      const b200z_zip_entry &e = entries[i];
+      const uint64_t k = std::min(out_len[i], out_room[i]);
+      if (e.has_data && !(e.flags & 1u) && e.method != 12 && k) cp.push_back(SlotCopy{out_off[i] - lo, out_off[i], k});
+    }
+    CU(copy_slots((const uint8_t *)g.d_out.p, out, cp.data(), cp.size(), g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+  } else if (any_dev) {
     if (hi > early_to)
-      CU(cudaMemcpyAsync(out + early_to, (const uint8_t *)g.d_out.p + early_to, hi - early_to, cudaMemcpyDeviceToHost, g.stream));
+      CU(cudaMemcpyAsync(out + early_to, (const uint8_t *)g.d_out.p + (early_to - lo), hi - early_to, cudaMemcpyDeviceToHost,
+                         g.stream));
     CU(cudaStreamSynchronize(g.stream));
     if (early_to > lo) CU(cudaStreamSynchronize(g.s_d2h));
   }
@@ -3414,7 +3435,7 @@ static int zip_extract_core(const uint8_t *z, size_t len, const b200z_zip_entry 
       const size_t i = bz_idx[k];
       jobs[k] = Bz2Job{entries[i].data_off, entries[i].comp_size, out + out_off[i], (size_t)out_room[i], 0, B200Z_OK};
     }
-    rc = bzip2_decode_device((const uint8_t *)g.d_in.p, jobs.data(), jobs.size(), 0);
+    rc = bzip2_decode_device((const uint8_t *)g.d_in.p, jobs.data(), jobs.size(), 0, nullptr, dev_out ? out : nullptr);
     if (rc) return rc;
     for (size_t k = 0; k < bz_idx.size(); ++k) {
       const size_t i = bz_idx[k];
@@ -3519,7 +3540,7 @@ struct CryptLayout {
 
 static int zip_extract_crypt(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                              size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
-                             int32_t *status, uint32_t flags, const uint8_t *pw, size_t pw_len) {
+                             int32_t *status, uint32_t flags, const uint8_t *pw, size_t pw_len, bool dev_out) {
   // 1. which members are encrypted how, and where their plaintext goes: the plaintext area starts behind the archive in
   //    g.d_in, every member is followed by >= 64 zero bytes (the inflate look-ahead reads zeros, as the oracle's does)
   std::vector<b200z_zip_entry> ve(entries, entries + n);
@@ -3579,7 +3600,7 @@ static int zip_extract_crypt(const uint8_t *z, size_t len, const b200z_zip_entry
     p = align_up(p + plen + 64, 256);
   }
   if (aes.empty() && zc.empty()) {
-    int rc = zip_extract_core(z, len, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr);
+    int rc = zip_extract_core(z, len, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr, dev_out);
     for (size_t i = 0; i < n && rc == B200Z_OK; ++i)
       if (forced[i] != 1) {
         status[i] = forced[i];
@@ -3653,7 +3674,7 @@ static int zip_extract_crypt(const uint8_t *z, size_t len, const b200z_zip_entry
   }
   // 5. every member kind sees the decrypted members as ranges of the staged buffer
   const ZipPlain pl{staged, len};
-  int rc = zip_extract_core(z, staged, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, &pl);
+  int rc = zip_extract_core(z, staged, ve.data(), n, out, out_cap, out_off, out_room, out_len, status, flags, &pl, dev_out);
   if (rc) {
     cudaStreamSynchronize(s_mac);
     return rc;
@@ -3700,9 +3721,81 @@ extern "C" int b200z_zip_extract_password(const uint8_t *z, size_t len, const b2
   if (!entries || !out_off || !out_room || !out_len || !status) return B200Z_E_ARG;
   std::lock_guard<std::mutex> lk(g.mu);
   CU(cudaSetDevice(g.device));
-  if (!password) return zip_extract_core(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr);
-  return zip_extract_crypt(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, password, password_len);
+  if (!password)
+    return zip_extract_core(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, nullptr, false);
+  return zip_extract_crypt(z, len, entries, n, out, out_cap, out_off, out_room, out_len, status, flags, password, password_len,
+                           false);
 }
+
+// crc32[i] = getCrc32 of the bytes member i delivered, d_out[out_off[i], + min(out_len[i], out_room[i])) (0 for a
+// B200Z_U_NOSPC member): the 8 KiB tiles of all members in one k_crc_tiles launch, folded per member on the host
+static int zip_slot_crc32(const uint8_t *d_out, const uint64_t *out_off, const uint64_t *out_room, const uint64_t *out_len,
+                          const int32_t *status, size_t n, uint32_t *crc32) {
+  const uint64_t TILE = kCrcTile;
+  std::vector<uint64_t> t_off;
+  std::vector<uint32_t> t_len;
+  std::vector<size_t> first(n + 1, 0);
+  for (size_t i = 0; i < n; ++i) {
+    first[i] = t_off.size();
+    const uint64_t k = status[i] == B200Z_U_NOSPC ? 0 : std::min(out_len[i], out_room[i]);
+    for (uint64_t o = 0; o < k; o += TILE) {
+      t_off.push_back(out_off[i] + o);
+      t_len.push_back((uint32_t)std::min(TILE, k - o));
+    }
+  }
+  first[n] = t_off.size();
+  const size_t nt = t_off.size();
+  std::vector<uint32_t> part(nt);
+  if (nt) {
+    const size_t o_len = align_up(nt * 8, 256), o_part = align_up(o_len + nt * 4, 256);
+    CU(g.d_small.reserve(o_part + nt * 4));
+    uint8_t *m = (uint8_t *)g.d_small.p;
+    CU(cudaMemcpyAsync(m, t_off.data(), nt * 8, cudaMemcpyHostToDevice, g.stream));
+    CU(cudaMemcpyAsync(m + o_len, t_len.data(), nt * 4, cudaMemcpyHostToDevice, g.stream));
+    CU(crc32_tiles_launch(d_out, (const uint64_t *)m, (const uint32_t *)(m + o_len), (uint32_t)nt, (uint32_t *)(m + o_part),
+                          g.stream));
+    CU(cudaMemcpyAsync(part.data(), m + o_part, nt * 4, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+  }
+  const uint32_t xfull = crc_xpow8(TILE);
+  for (size_t i = 0; i < n; ++i) {
+    uint32_t c = 0;  // the CRC of nothing
+    for (size_t t = first[i]; t < first[i + 1]; ++t) c = crc_multmodp(t_len[t] == TILE ? xfull : crc_xpow8(t_len[t]), c) ^ part[t];
+    crc32[i] = c;
+  }
+  return B200Z_OK;
+}
+
+extern "C" int b200z_zip_extract_to_device(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n,
+                                           uint8_t *d_out, size_t out_cap, const uint64_t *out_off, const uint64_t *out_room,
+                                           uint64_t *out_len, int32_t *status, uint32_t *crc32, uint32_t flags,
+                                           const uint8_t *password, size_t password_len, void *cuda_stream) {
+  int rc = require_init();
+  if (rc) return rc;
+  if (n == 0) return B200Z_OK;
+  if (!entries || !out_off || !out_room || !out_len || !status) return B200Z_E_ARG;
+  if ((rc = device_out_arg("zip_extract_to_device", d_out, n, out_room)) != B200Z_OK) return rc;
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  if ((rc = wait_for_caller(cuda_stream)) != B200Z_OK) return rc;
+  // results go to the caller's arrays only once the call has succeeded, so that an argument error writes nothing
+  std::vector<uint64_t> r_len(n);
+  std::vector<int32_t> r_st(n);
+  std::vector<uint32_t> r_crc(crc32 ? n : 0);
+  rc = password ? zip_extract_crypt(z, len, entries, n, d_out, out_cap, out_off, out_room, r_len.data(), r_st.data(), flags,
+                                    password, password_len, true)
+                : zip_extract_core(z, len, entries, n, d_out, out_cap, out_off, out_room, r_len.data(), r_st.data(), flags,
+                                   nullptr, true);
+  if (rc == B200Z_OK && crc32) rc = zip_slot_crc32(d_out, out_off, out_room, r_len.data(), r_st.data(), n, r_crc.data());
+  if (rc) return rc;
+  memcpy(out_len, r_len.data(), n * 8);
+  memcpy(status, r_st.data(), n * 4);
+  if (crc32) memcpy(crc32, r_crc.data(), n * 4);
+  return B200Z_OK;
+}
+
+// (test hook) the g.d_out bytes the last b200z_zip_extract* call asked for: the slots' span, not their end
+extern "C" uint64_t b200z_debug_zip_out_bytes(void) { return g_zip_out_bytes; }
 
 extern "C" int b200z_zip_extract(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                                  size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,

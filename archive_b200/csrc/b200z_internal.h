@@ -234,6 +234,10 @@ size_t xz_bound(const uint8_t *in, size_t n);  // the output the container decla
 int xz_decode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int verify,
                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
                       cudaStream_t s, bool dev_out = false);
+// CRC-32 (getCrc32) of each tile d[tile_off[t], + tile_len[t]) into part[t]: one k_crc_tiles<uint32_t> launch on s, not
+// synchronised (nothing when n_tiles == 0); the caller folds the tiles of a range with the x^(8n) mod P combine
+cudaError_t crc32_tiles_launch(const uint8_t *d, const uint64_t *tile_off, const uint32_t *tile_len, uint32_t n_tiles,
+                               uint32_t *part, cudaStream_t s);
 int xz_encode_streams(const uint8_t *in_base, const uint64_t *in_off, const uint64_t *in_len, size_t n, int check,
                       uint8_t *out_base, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_len, int32_t *rc,
                       cudaStream_t s);

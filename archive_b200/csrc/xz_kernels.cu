@@ -412,6 +412,14 @@ __global__ void __launch_bounds__(256) k_crc_tiles(const uint8_t *__restrict__ d
   part[t] = ~c;
 }
 
+cudaError_t crc32_tiles_launch(const uint8_t *d, const uint64_t *tile_off, const uint32_t *tile_len, uint32_t n_tiles,
+                               uint32_t *part, cudaStream_t s) {
+  if (!n_tiles) return cudaSuccess;
+  XZ_LAUNCH(k_crc_tiles<uint32_t>, (n_tiles + 255) / 256, 256, s, d, tile_off, tile_len, n_tiles, XZ_POLY32, part);
+  count_launch();
+  return cudaGetLastError();
+}
+
 __device__ __forceinline__ uint32_t xz_ror(uint32_t x, int n) { return (x >> n) | (x << (32 - n)); }
 __constant__ uint32_t c_k256[64] = {
     0x428a2f98, 0x71374491, 0xb5c0fbcf, 0xe9b5dba5, 0x3956c25b, 0x59f111f1, 0x923f82a4, 0xab1c5ed5, 0xd807aa98, 0x12835b01,

@@ -205,7 +205,7 @@ def zip_extract_sharded(data, rank: int, world: int, web_eos: bool = False):
     import ctypes as C
     from . import _ffi
     sub = (_ffi.ZipEntry * len(mine))(*[ents[i] for i in mine])
-    contents, statuses = dec._extract(data, sub, len(mine))
+    contents = dec._extract(data, sub, len(mine))[0]
     return ents, {i: contents[k] for k, i in enumerate(mine)}
 
 

@@ -55,6 +55,7 @@ class ArchiveFile:
         self.content = b"" if is_file else None
         self.status = U_DONE  # unit status of the member's decode (include/b200z.h)
         self.encrypted = False  # decrypted with a password (the errors below are then the reference's throws)
+        self._computed_crc32 = None  # ZipFile._computedCrc32: set by a device extract, else computed on first use
 
     @property
     def is_symbolic_link(self):
@@ -64,6 +65,20 @@ class ArchiveFile:
         if self.encrypted and self.status in _CRYPT_ERRORS:  # ZipFile.getStream throws on access (zip_file.dart:333-341)
             raise ArchiveException(f"{self.name}: {_CRYPT_ERRORS[self.status]}")
         return self.content
+
+    def verify_crc32(self) -> bool:
+        """ZipFile.verifyCrc32 (zip_file.dart:157-161): getCrc32 of the content against `crc32`.  Content extracted to a
+        device carries the CRC its extract call computed there; host content is hashed with b200z_crc32."""
+        data = self.read_bytes()
+        if self._computed_crc32 is None:
+            data = bytes(data or b"")
+            crc = C.c_uint32(0)
+            if data:
+                L = _ffi.ensure_init()
+                addr, n, keep = _ffi.as_buffer(data)
+                _ffi.check(L.b200z_crc32(addr, n, C.byref(crc)))
+            self._computed_crc32 = crc.value
+        return self._computed_crc32 == self.crc32
 
 
 class Archive:
@@ -113,7 +128,7 @@ class ZipDecoder:
         self.zip_file_comment = raw.decode("latin-1")  # readString(utf8: false) (zip_directory.dart:43)
         return ents, cnt.value
 
-    def decode_stream(self, input, verify: bool = False, password=None) -> Archive:
+    def decode_stream(self, input, verify: bool = False, password=None, device=None) -> Archive:
         """ZipDecoder().decodeStream(input) (zip_decoder.dart:29-81): the rest of an InputMemoryStream or InputFileStream."""
         from .streams import InputFileStream
         if isinstance(input, InputFileStream):
@@ -122,7 +137,7 @@ class ZipDecoder:
         else:
             data = bytes(input.buffer[input.position:])
             input.position = len(input.buffer)
-        return self.decode_bytes(data, verify=verify, password=password)
+        return self.decode_bytes(data, verify=verify, password=password, device=device)
 
     def crypt_info(self, data, entry):
         """-> (mode CRYPT_*, AES strength byte, method the content is stored with), as ZipFile.read decides
@@ -133,13 +148,17 @@ class ZipDecoder:
         _ffi.check(L.b200z_zip_crypt_info(addr, n, C.byref(entry), C.byref(mode), C.byref(strength), C.byref(method)))
         return mode.value, strength.value, method.value
 
-    def decode_bytes(self, data, verify: bool = False, password=None) -> Archive:
+    def decode_bytes(self, data, verify: bool = False, password=None, device=None) -> Archive:
         """password: str (Dart's code units cut to 8 bits, see password_bytes) or bytes.  Without one, encrypted members
-        keep status ZIP_ENCRYPTED and empty content."""
+        keep status ZIP_ENCRYPTED and empty content.  verify does nothing, as in the reference (its check is commented
+        out); ArchiveFile.verify_crc32 makes it.
+        device: None (content is bytes), or the library's torch CUDA device: every member goes straight into one CUDA
+        buffer per call (b200z_zip_extract_to_device, ordered after torch.cuda.current_stream()), each file's content is a
+        uint8 tensor view into it, and the member CRC-32s are computed there.  Any other device raises ValueError."""
         data = bytes(data) if not isinstance(data, (bytes, bytearray)) else data
         pw = password_bytes(password)
         ents, n = self.list(data)
-        contents, statuses = self._extract(data, ents, n, pw)
+        contents, statuses, crcs = self._extract(data, ents, n, pw, device)
         archive = Archive()
         for i in range(n):
             e = ents[i]
@@ -156,7 +175,7 @@ class ZipDecoder:
                         pass
                 entry.compression = COMPRESSION.get(method, "none") if e.has_data else "none"
                 if not is_dir:
-                    entry.content, entry.status = contents[i], statuses[i]
+                    entry.content, entry.status, entry._computed_crc32 = contents[i], statuses[i], crcs[i]
                     entry.encrypted = pw is not None and bool(e.has_data and (e.flags & 1))
                 archive.add(entry)
             entry.mode = e.ext_attr >> 16
@@ -164,21 +183,27 @@ class ZipDecoder:
                 if pw is not None and e.has_data and (e.flags & 1) and statuses[i] in _CRYPT_ERRORS:
                     # decodeStream reads a symlink's content while it walks the directory: the throw happens here
                     raise ArchiveException(f"{name}: {_CRYPT_ERRORS[statuses[i]]}")
-                try:
-                    entry.symbolic_link = contents[i].decode("utf-8")
+                try:  # (a device member's target is read back: the walk needs it on the host)
+                    target = contents[i] if device is None else bytes(contents[i].cpu().numpy())
+                    entry.symbolic_link = target.decode("utf-8")
                 except UnicodeDecodeError:
                     pass
             entry.crc32 = e.crc32
             entry.last_mod_time = (e.mod_date << 16) | e.mod_time
         return archive
 
-    def _extract(self, data, ents, n, password=None):
+    def _extract(self, data, ents, n, password=None, device=None):
+        """-> (contents, statuses, crcs): crcs[i] is the member's CRC-32 when the device call computed it, else None."""
+        from .codecs import _Sink
+        sink = _Sink(device)
         if n == 0:
-            return [], []
+            return [], [], []
         L = _ffi.ensure_init()
         addr, zlen, keep = _ffi.as_buffer(data)
         room = [max(int(ents[i].hint_uncomp_size), int(ents[i].uncomp_size), 1) if ents[i].has_data else 0 for i in range(n)]
-        contents, statuses = [b""] * n, [U_DONE] * n
+        contents, statuses, crcs = [b""] * n, [U_DONE] * n, [None] * n
+        if sink.torch is not None:
+            contents = [sink.torch.empty(0, dtype=sink.torch.uint8, device=sink.device)] * n
         todo = list(range(n))
         while todo:
             m = len(todo)
@@ -186,13 +211,20 @@ class ZipDecoder:
             off, tot = [], 0
             for i in todo:
                 off.append(tot)
-                tot += (room[i] + 63) & ~63
-            out = (C.c_uint8 * max(tot, 1))()
+                tot += (room[i] + 63) & ~63 if sink.torch is None else sink.room(room[i])
+            out, out_addr = sink.alloc(tot)
             a64 = lambda l: (C.c_uint64 * m)(*l)
             out_len, st = (C.c_uint64 * m)(), (C.c_int32 * m)()
-            _ffi.check(L.b200z_zip_extract_password(addr, zlen, sub, m, C.addressof(out), max(tot, 1), a64(off),
-                                                    a64([room[i] for i in todo]), out_len, st, self.flags, password,
-                                                    len(password or b"")))
+            crc = None
+            if sink.torch is None:
+                _ffi.check(L.b200z_zip_extract_password(addr, zlen, sub, m, out_addr, max(tot, 1), a64(off),
+                                                        a64([room[i] for i in todo]), out_len, st, self.flags, password,
+                                                        len(password or b"")))
+            else:
+                crc = (C.c_uint32 * m)()
+                _ffi.check(L.b200z_zip_extract_to_device(addr, zlen, sub, m, out_addr, max(tot, 1), a64(off),
+                                                         a64([room[i] for i in todo]), out_len, st, crc, self.flags,
+                                                         password, len(password or b""), sink.stream))
             again = []
             for k, i in enumerate(todo):
                 statuses[i] = st[k]
@@ -200,9 +232,11 @@ class ZipDecoder:
                     room[i] = min(max(room[i] * 4, int(out_len[k]), int(ents[i].comp_size) * 4), (1 << 32) - 64)
                     again.append(i)
                     continue
-                contents[i] = C.string_at(C.addressof(out) + off[k], min(int(out_len[k]), room[i]))
+                contents[i] = sink.take(out, off[k], min(int(out_len[k]), room[i]))
+                if crc is not None:
+                    crcs[i] = crc[k]
             todo = again
-        return contents, statuses
+        return contents, statuses, crcs
 
 
 # ---------------------------------------------------------------------------------------------

@@ -171,6 +171,14 @@ typedef _ZipExtractPasswordC = Int32 Function(Pointer<Uint8> zip, Size zipLen, P
 typedef _ZipExtractPasswordD = int Function(Pointer<Uint8> zip, int zipLen, Pointer<ZipEntry> entries, int n,
     Pointer<Uint8> out, int outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen,
     Pointer<Int32> status, int flags, Pointer<Uint8> password, int passwordLen);
+typedef _ZipExtractToDeviceC = Int32 Function(Pointer<Uint8> zip, Size zipLen, Pointer<ZipEntry> entries, Size n,
+    Pointer<Uint8> dOut, Size outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen,
+    Pointer<Int32> status, Pointer<Uint32> crc32, Uint32 flags, Pointer<Uint8> password, Size passwordLen,
+    Pointer<Void> cudaStream);
+typedef _ZipExtractToDeviceD = int Function(Pointer<Uint8> zip, int zipLen, Pointer<ZipEntry> entries, int n,
+    Pointer<Uint8> dOut, int outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen,
+    Pointer<Int32> status, Pointer<Uint32> crc32, int flags, Pointer<Uint8> password, int passwordLen,
+    Pointer<Void> cudaStream);
 typedef _ZipAesEncryptC = Int32 Function(Pointer<Uint8> data, Pointer<Uint64> off, Pointer<Uint64> len, Size n,
     Pointer<Uint8> salts, Pointer<Uint8> password, Size passwordLen, Pointer<Uint8> pwdVerify, Pointer<Uint8> mac);
 typedef _ZipAesEncryptD = int Function(Pointer<Uint8> data, Pointer<Uint64> off, Pointer<Uint64> len, int n,
@@ -291,6 +299,9 @@ class B200Z {
   late final _ZipCryptInfoD zipCryptInfo = _lib.lookupFunction<_ZipCryptInfoC, _ZipCryptInfoD>('b200z_zip_crypt_info');
   late final _ZipExtractPasswordD zipExtractPassword =
       _lib.lookupFunction<_ZipExtractPasswordC, _ZipExtractPasswordD>('b200z_zip_extract_password');
+  // dOut: device memory of the library's device; crc32 may be nullptr
+  late final _ZipExtractToDeviceD zipExtractToDevice =
+      _lib.lookupFunction<_ZipExtractToDeviceC, _ZipExtractToDeviceD>('b200z_zip_extract_to_device');
   late final _ZipAesEncryptD zipAesEncrypt = _lib.lookupFunction<_ZipAesEncryptC, _ZipAesEncryptD>('b200z_zip_aes_encrypt');
   late final _Bz2ShardD bzip2DecodeShard = _lib.lookupFunction<_Bz2ShardC, _Bz2ShardD>('b200z_bzip2_decode_shard');
   late final _Crc32D crc32 = _lib.lookupFunction<_Crc32C, _Crc32D>('b200z_crc32');

@@ -314,6 +314,28 @@ int b200z_zip_crypt_info(const uint8_t *zip, size_t zip_len, const b200z_zip_ent
 int b200z_zip_extract_password(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                                size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
                                int32_t *status, uint32_t flags, const uint8_t *password, size_t password_len);
+/* b200z_zip_extract_to_device = b200z_zip_extract_password (password == NULL: b200z_zip_extract) with the member slots in
+ * device memory, so that decoded members never make the round trip through the host.
+ *   Memory: `zip`, `entries` and every array are host memory; d_out is device memory on the b200z_init device.
+ *   Results: for every member, status[i], out_len[i] and the bytes d_out[out_off[i] .. + min(out_len[i], out_room[i])) are
+ *     exactly what the host call gives for the same arguments; slot contents beyond that, and the whole slot of a
+ *     B200Z_U_NOSPC member, are unspecified, as on the host.
+ *     Nothing is written outside the slots; slots may come in any order, leave gaps and start at any byte alignment.
+ *   crc32 (may be NULL): crc32[i] = getCrc32 of member i's delivered bytes, computed on the device over the slot after
+ *     delivery (0 for members without data and for B200Z_U_NOSPC members) -- what ZipFile.verifyCrc32 compares.
+ *   Argument errors: the host call's rules, and d_out must be device memory of the library's device
+ *     (cudaPointerGetAttributes) whenever a member has room: B200Z_E_ARG.  No device: B200Z_E_NODEVICE.  On any error
+ *     nothing is written, neither to d_out nor to out_len / status / crc32.
+ *   Ordering: the library's stream waits on an event recorded on cuda_stream (a cudaStream_t; NULL = the library's own
+ *     stream, cudaStreamLegacy for the legacy default stream) when the call starts, and the call returns once the bytes are
+ *     in place, as the *_decode_batch_to_device calls do.
+ * Members decode into the library's buffer as in the host call (sized by the slots' span, not their end), and reach their
+ * slots with one k_copy_slots launch for all deflate / stored members plus the BZip2 batch's own deliveries; the CRCs take
+ * one launch more.  The launch count does not grow with the member count.                                          */
+int b200z_zip_extract_to_device(const uint8_t *zip, size_t zip_len, const b200z_zip_entry *entries, size_t n, uint8_t *d_out,
+                                size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
+                                int32_t *status, uint32_t *crc32, uint32_t flags, const uint8_t *password,
+                                size_t password_len, void *cuda_stream);
 /* ZipEncoder(password:) member payloads (zip_encoder.dart:166-183): AES-256 in place on host buffers.  Member i is
  * data[off[i] .. +len[i]) (already compressed), salts[16 i ..] its salt; on return it is the ciphertext,
  * pwd_verify[2 i ..] its password verifier and mac[10 i ..] the first 10 bytes of the HMAC-SHA1 of the ciphertext.  An

@@ -6,5 +6,5 @@ from .codecs import XZCheck, XZDecoder, XZEncoder, bzip2_decode_batch, get_crc64
 from .codecs import gzip_decode_batch, gzip_encode_batch, zlib_decode_batch, zlib_encode_batch  # noqa: F401
 from .streams import BIG_ENDIAN, LITTLE_ENDIAN, InputFileStream, InputMemoryStream, OutputFileStream, OutputMemoryStream  # noqa: F401
 from .zip import Archive, ArchiveFile, ZipDecoder, ZipEncoder, bzip2_encode_batch  # noqa: F401,E402
-from .tar import TarDecoder, TarEncoder, TarFile  # noqa: F401,E402
+from .tar import TarDecoder, TarEncoder, TarFile, tar_decode_batch  # noqa: F401,E402
 from .io import TarFileEncoder, ZipFileEncoder, extract_archive_to_disk, extract_file_to_disk, get_input_extension  # noqa: F401,E402

@@ -49,6 +49,12 @@ class ZipEntry(C.Structure):
                 ("ext_attr", C.c_uint32), ("version_made_by", C.c_uint32), ("has_data", C.c_uint32)]
 
 
+class TarMember(C.Structure):
+    """b200z_tar_member (include/b200z.h)"""
+    _fields_ = [("header_off", C.c_uint64), ("content_off", C.c_uint64), ("content_len", C.c_uint64), ("size", C.c_int64),
+                ("header_len", C.c_uint32), ("pad_", C.c_uint32)]
+
+
 _SIGS = {
     "b200z_init": (C.c_int, [C.c_int, C.c_uint32]),
     "b200z_shutdown": (None, []),
@@ -117,6 +123,9 @@ _SIGS = {
     "b200z_zip_extract_to_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                               C.c_size_t, C.c_void_p]),
+    # the TAR member walk over archives in device memory, plus the caller's cudaStream_t
+    "b200z_tar_walk_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t), C.c_void_p]),
     "b200z_zip_aes_encrypt": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
                                         C.c_void_p, C.c_void_p]),
     "b200z_bzip2_decode_shard": (C.c_int, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t,

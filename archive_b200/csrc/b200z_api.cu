@@ -3797,6 +3797,296 @@ extern "C" int b200z_zip_extract_to_device(const uint8_t *z, size_t len, const b
 // (test hook) the g.d_out bytes the last b200z_zip_extract* call asked for: the slots' span, not their end
 extern "C" uint64_t b200z_debug_zip_out_bytes(void) { return g_zip_out_bytes; }
 
+// ---------------------------------------------------------------------------------------------
+// TAR member walk (b200z_tar_walk_device): TarDecoder._decode's loop with storeData (tar_decoder.dart:28-38) and the
+// position arithmetic of TarFile.read (tar_file.dart:74-118, input_memory_stream.dart:96-119).  A header's size field
+// says where the next header is, so the walk is a dependent chain of loads, one per member.  One warp per archive: the
+// bytes a member's step needs (the first two, the size field and the type byte) are one load per lane, then every lane
+// parses the field the same way and lane 0 writes the record.
+// ---------------------------------------------------------------------------------------------
+constexpr unsigned TAR_THREADS = 128;
+static cudaEvent_t g_tar_ev[2] = {nullptr, nullptr};  // created once, kept for the life of the library
+static double g_tar_walk_ms = 0;  // k_tar_walk of the last call, by CUDA events (b200z_debug_tar_walk)
+struct TarArchive {
+  uint64_t off, len;  // the archive, from the call's d_base
+  uint64_t rec;       // its first record slot in the workspace (the prefix sum of the bounds len / 512 + 1)
+};
+struct TarCount {
+  uint64_t count, first;  // members, and where they start in the gathered area
+  int32_t rc, pad_;
+};
+
+__device__ __forceinline__ uint32_t tar_fb(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t i) {
+  return ((i < 4 ? w0 : i < 8 ? w1 : w2) >> (8 * (i & 3))) & 0xffu;
+}
+// a three-byte UTF-8 form of a character Dart's trim removes: U+1680, U+2000-200A, U+2028/9, U+202F, U+205F, U+3000, U+FEFF
+__device__ __forceinline__ bool tar_ws3(uint32_t a, uint32_t b, uint32_t c) {
+  return (a == 0xE1 && b == 0x9A && c == 0x80) ||
+         (a == 0xE2 && b == 0x80 && ((c >= 0x80 && c <= 0x8A) || c == 0xA8 || c == 0xA9 || c == 0xAF)) ||
+         (a == 0xE2 && b == 0x81 && c == 0x9F) || (a == 0xE3 && b == 0x80 && c == 0x80) || (a == 0xEF && b == 0xBB && c == 0xBF);
+}
+__device__ __forceinline__ bool tar_ascii_ws(uint32_t c) { return c == 0x20 || (c >= 0x09 && c <= 0x0D); }
+
+// _parseInt (tar_file.dart:211-225) of the field's first n bytes (already cut at the first NUL): decoded as UTF-8 when the
+// bytes are valid UTF-8 (Python's strict decoder: no overlong forms, surrogates or code points past U+10FFFF), else as
+// Latin-1; Dart's trim at both ends; then int.parse(radix: 8), which takes [+-]?[0-7]+ and nothing else (0 otherwise)
+__device__ int64_t tar_parse_size(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t n) {
+  bool utf8 = true;
+  for (uint32_t i = 0; i < n && utf8;) {
+    const uint32_t c = tar_fb(w0, w1, w2, i);
+    if (c < 0x80) {
+      ++i;
+      continue;
+    }
+    const uint32_t need = c < 0xC2 ? 0 : c < 0xE0 ? 1 : c < 0xF0 ? 2 : c < 0xF5 ? 3 : 0;
+    if (need == 0 || i + need >= n) {  // not a lead byte, or the sequence is cut short
+      utf8 = false;
+      break;
+    }
+    const uint32_t lo = c == 0xE0 ? 0xA0 : c == 0xF0 ? 0x90 : 0x80, hi = c == 0xED ? 0x9F : c == 0xF4 ? 0x8F : 0xBF;
+    const uint32_t c1 = tar_fb(w0, w1, w2, i + 1);
+    utf8 = c1 >= lo && c1 <= hi;
+    for (uint32_t k = 2; k <= need && utf8; ++k) {
+      const uint32_t ck = tar_fb(w0, w1, w2, i + k);
+      utf8 = ck >= 0x80 && ck <= 0xBF;
+    }
+    i += need + 1;
+  }
+  uint32_t l = 0, r = n;
+  while (l < r) {  // the left end
+    const uint32_t c = tar_fb(w0, w1, w2, l);
+    uint32_t k = 0;
+    if (tar_ascii_ws(c)) k = 1;
+    else if (!utf8) k = c == 0x85 || c == 0xA0 ? 1 : 0;
+    else if (c == 0xC2 && l + 1 < r) k = tar_fb(w0, w1, w2, l + 1) == 0x85 || tar_fb(w0, w1, w2, l + 1) == 0xA0 ? 2 : 0;
+    else if (l + 2 < r && tar_ws3(c, tar_fb(w0, w1, w2, l + 1), tar_fb(w0, w1, w2, l + 2))) k = 3;
+    if (k == 0) break;
+    l += k;
+  }
+  while (r > l) {  // the right end (valid UTF-8: a lead byte at r - 2 or r - 3 starts the last character)
+    const uint32_t c = tar_fb(w0, w1, w2, r - 1);
+    uint32_t k = 0;
+    if (tar_ascii_ws(c)) k = 1;
+    else if (!utf8) k = c == 0x85 || c == 0xA0 ? 1 : 0;
+    else if (r - l >= 2 && tar_fb(w0, w1, w2, r - 2) == 0xC2 && (c == 0x85 || c == 0xA0)) k = 2;
+    else if (r - l >= 3 && tar_ws3(tar_fb(w0, w1, w2, r - 3), tar_fb(w0, w1, w2, r - 2), c)) k = 3;
+    if (k == 0) break;
+    r -= k;
+  }
+  bool neg = false;
+  if (l < r) {
+    const uint32_t c = tar_fb(w0, w1, w2, l);
+    if (c == '+' || c == '-') {
+      neg = c == '-';
+      ++l;
+    }
+  }
+  if (l >= r) return 0;  // nothing, or a sign alone
+  int64_t v = 0;
+  for (uint32_t i = l; i < r; ++i) {
+    const uint32_t c = tar_fb(w0, w1, w2, i);
+    if (c < '0' || c > '7') return 0;
+    v = v * 8 + (c - '0');  // at most 12 digits: below 2^36
+  }
+  return neg ? -v : v;
+}
+
+// rec: the records at each archive's bound slots.  When its walk ends, the warp takes the next count slots of the gathered
+// area (one atomicAdd on *next) and writes a k_copy_slots piece for each header there: from d_from + off + header_off
+// (d_from: d_base from the launch's source base) to slot * 512.
+__global__ void __launch_bounds__(TAR_THREADS) k_tar_walk(const uint8_t *__restrict__ base, const TarArchive *__restrict__ ar,
+                                                          uint32_t n, b200z_tar_member *__restrict__ rec, TarCount *__restrict__ res,
+                                                          SlotCopy *__restrict__ pieces, unsigned long long *__restrict__ next,
+                                                          uint64_t d_from) {
+  const uint32_t lane = threadIdx.x & 31, w = blockIdx.x * (TAR_THREADS / 32) + (threadIdx.x >> 5);
+  if (w >= n) return;  // (the whole warp)
+  const TarArchive a = ar[w];
+  const uint8_t *D = base + a.off;
+  const uint64_t L = a.len, bound = L / 512 + 1;
+  b200z_tar_member *R = rec + a.rec;
+  // lanes 0-11: the size field (header bytes 124-135); lane 12: the type byte (156); lanes 13, 14: the first two bytes
+  const uint32_t at = lane < 12 ? 124 + lane : lane == 12 ? 156 : lane - 13;
+  uint64_t pos = 0, k = 0;
+  int32_t st = B200Z_OK;
+  while (pos < L) {
+    const uint64_t left = L - pos;
+    const int b = lane < 15 && at < left ? (int)D[pos + at] : -1;  // -1: past the archive's end
+    const int b0 = __shfl_sync(0xffffffffu, b, 13), b1 = __shfl_sync(0xffffffffu, b, 14);
+    if (b1 < 0 || (b0 == 0 && b1 == 0)) break;  // one byte left, or two zero bytes: the end (tar_decoder.dart:35-38)
+    if (k == bound) {  // (cannot happen: every member but the last takes 512 bytes or more)
+      st = B200Z_E_INTERNAL;
+      break;
+    }
+    const uint32_t hl = left < 512 ? (uint32_t)left : 512;
+    // the field: the bytes present, cut at the first NUL
+    const uint32_t present = __ballot_sync(0xffffffffu, lane < 12 && b >= 0), nul = __ballot_sync(0xffffffffu, lane < 12 && b == 0);
+    uint32_t fl = __popc(present);
+    if (nul) fl = min(fl, (uint32_t)(__ffs(nul) - 1));
+    const uint32_t v = b > 0 ? (uint32_t)b : 0;
+    uint32_t wd[3];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      uint32_t x = 0;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) x |= __shfl_sync(0xffffffffu, v, 4 * j + q) << (8 * q);
+      wd[j] = x;
+    }
+    const int64_t size = tar_parse_size(wd[0], wd[1], wd[2], fl);
+    if (size < 0) {  // readBytes of a negative count: RangeError
+      st = B200Z_E_THROW;
+      break;
+    }
+    const uint64_t content_off = pos + hl, clen = min((uint64_t)size, L - content_off);
+    if (lane == 0) {
+      b200z_tar_member m;
+      m.header_off = pos;
+      m.content_off = content_off;
+      m.content_len = clen;
+      m.size = size;
+      m.header_len = hl;
+      m.pad_ = 0;
+      R[k] = m;
+    }
+    ++k;
+    pos = content_off + clen;
+    const int type = __shfl_sync(0xffffffffu, b, 12);
+    if (type != '5' && size % 512 != 0) pos = min(pos + 512 - (uint64_t)(size % 512), L);  // (size 0: no padding)
+  }
+  unsigned long long first = 0;
+  if (lane == 0) first = atomicAdd(next, (unsigned long long)k);
+  first = __shfl_sync(0xffffffffu, first, 0);
+  __syncwarp();  // (lane 0's records, read back by every lane)
+  for (uint64_t j = lane; j < k; j += 32)
+    pieces[first + j] = SlotCopy{d_from + a.off + R[j].header_off, (first + j) * 512, R[j].header_len};
+  if (lane == 0) {
+    res[w].count = k;
+    res[w].first = first;
+    res[w].rc = st;
+    res[w].pad_ = 0;
+  }
+}
+
+extern "C" int b200z_tar_walk_device(const uint8_t *d_base, const uint64_t *off, const uint64_t *len, size_t n,
+                                     b200z_tar_member *members, uint8_t *headers, size_t cap, uint64_t *first, uint64_t *count,
+                                     int32_t *rc, size_t *n_total, void *cuda_stream) {
+  int r = require_init();
+  if (r) return r;
+  if (n == 0) {
+    if (n_total) *n_total = 0;
+    return B200Z_OK;
+  }
+  if (!off || !len || !first || !count || !rc || !n_total || (cap && (!members || !headers))) {
+    set_err("tar_walk_device: null array");
+    return B200Z_E_ARG;
+  }
+  uint64_t n_rec = 0;  // the record bound of the call
+  for (size_t i = 0; i < n; ++i) {
+    if (off[i] + len[i] < off[i] || (len[i] && !d_base)) {
+      set_err("tar_walk_device: archive %zu: bad range", i);
+      return B200Z_E_ARG;
+    }
+    for (int end = 0; end < 2 && len[i]; ++end) {  // the archive's first and last byte
+      cudaPointerAttributes pa;
+      if (cudaPointerGetAttributes(&pa, d_base + off[i] + (end ? len[i] - 1 : 0)) != cudaSuccess ||
+          pa.type != cudaMemoryTypeDevice || pa.device != g.device) {
+        cudaGetLastError();
+        set_err("tar_walk_device: archive %zu is not in device memory of device %d", i, g.device);
+        return B200Z_E_ARG;
+      }
+    }
+    n_rec += len[i] / 512 + 1;
+  }
+  std::lock_guard<std::mutex> lk(g.mu);
+  CU(cudaSetDevice(g.device));
+  if ((r = wait_for_caller(cuda_stream))) return r;
+  // g.d_ws: the archive table and the gathered-slot counter (one upload), the per-archive counts, the records at their
+  // bound slots, and the k_copy_slots pieces: one per member's header, then the records' pieces (one per archive and per
+  // COPY_PIECE bytes of records: at most n + n_rec * 40 / COPY_PIECE of them)
+  const size_t o_next = n * sizeof(TarArchive), o_cnt = align_up(o_next + 8, 256);
+  const size_t o_rec = o_cnt + align_up(n * sizeof(TarCount), 256);
+  const size_t o_pc = o_rec + align_up(n_rec * sizeof(b200z_tar_member), 256);
+  const size_t ws_bytes = o_pc + (n_rec + n + n_rec * sizeof(b200z_tar_member) / COPY_PIECE + 1) * sizeof(SlotCopy);
+  std::vector<uint8_t> up(o_next + 8, 0);
+  TarArchive *tab = (TarArchive *)up.data();
+  for (size_t i = 0, at = 0; i < n; at += len[i] / 512 + 1, ++i) tab[i] = TarArchive{off[i], len[i], at};
+  CU(g.d_ws.reserve(ws_bytes));
+  uint8_t *ws = (uint8_t *)g.d_ws.p;
+  // one source base for k_copy_slots: the lower of d_base and the workspace (headers come from the one, records from the other)
+  const uint8_t *src = d_base && d_base < ws ? d_base : ws;
+  CU(cudaMemcpyAsync(ws, up.data(), up.size(), cudaMemcpyHostToDevice, g.stream));
+  const unsigned per_cta = TAR_THREADS / 32;
+  if (!g_tar_ev[0]) {
+    CU(cudaEventCreate(&g_tar_ev[0]));
+    CU(cudaEventCreate(&g_tar_ev[1]));
+  }
+  CU(cudaEventRecord(g_tar_ev[0], g.stream));
+  k_tar_walk<<<(unsigned)((n + per_cta - 1) / per_cta), TAR_THREADS, 0, g.stream>>>(
+      d_base, (const TarArchive *)ws, (uint32_t)n, (b200z_tar_member *)(ws + o_rec), (TarCount *)(ws + o_cnt),
+      (SlotCopy *)(ws + o_pc), (unsigned long long *)(ws + o_next), d_base ? (uint64_t)(d_base - src) : 0);
+  count_launch();
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(g_tar_ev[1], g.stream));
+  std::vector<TarCount> cnt(n);
+  CU(cudaMemcpyAsync(cnt.data(), ws + o_cnt, n * sizeof(TarCount), cudaMemcpyDeviceToHost, g.stream));
+  CU(cudaStreamSynchronize(g.stream));
+  float walk_ms = 0;
+  CU(cudaEventElapsedTime(&walk_ms, g_tar_ev[0], g_tar_ev[1]));
+  g_tar_walk_ms = walk_ms;
+  uint64_t total = 0;
+  std::vector<uint64_t> at_first(n);  // archive i's members start at the exclusive prefix sum of the counts
+  for (size_t i = 0; i < n; ++i) {
+    if (cnt[i].rc == B200Z_E_INTERNAL) {
+      set_err("tar_walk_device: archive %zu has more members than its bound", i);
+      return B200Z_E_INTERNAL;
+    }
+    at_first[i] = total;
+    total += cnt[i].count;
+  }
+  if (total > cap) {
+    set_err("tar_walk_device: %llu members, cap %zu", (unsigned long long)total, cap);
+    *n_total = (size_t)total;
+    return B200Z_E_NOSPC;
+  }
+  if (total) {
+    // g.d_out: the gathered area, every header (512 bytes each, in the slots the warps took) and then the records (in
+    // archive order); one k_copy_slots takes the header pieces the walk wrote and the records' pieces, and the area comes
+    // back in one copy through the pinned staging buffer.  The host puts each archive's headers in archive order.
+    const size_t o_recs = total * 512, out_bytes = o_recs + total * sizeof(b200z_tar_member);
+    std::vector<SlotCopy> rp;
+    for (size_t i = 0; i < n; ++i) {
+      const uint64_t from = (uint64_t)(ws - src) + o_rec + tab[i].rec * sizeof(b200z_tar_member);
+      const uint64_t to = o_recs + at_first[i] * sizeof(b200z_tar_member), bytes = cnt[i].count * sizeof(b200z_tar_member);
+      for (uint64_t at = 0; at < bytes; at += COPY_PIECE) rp.push_back(SlotCopy{from + at, to + at, std::min(COPY_PIECE, bytes - at)});
+    }
+    const size_t n_pc = total + rp.size();
+    CU(cudaMemcpyAsync(ws + o_pc + total * sizeof(SlotCopy), rp.data(), rp.size() * sizeof(SlotCopy), cudaMemcpyHostToDevice,
+                       g.stream));
+    CU(g.d_out.reserve(out_bytes));
+    const unsigned grid = (unsigned)std::min<size_t>((n_pc + COPY_THREADS / 32 - 1) / (COPY_THREADS / 32), 1u << 16);
+    k_copy_slots<<<grid, COPY_THREADS, 0, g.stream>>>(src, (uint8_t *)g.d_out.p, (const SlotCopy *)(ws + o_pc), (uint32_t)n_pc);
+    count_launch();
+    CU(cudaGetLastError());
+    CU(g.h_stage.reserve(out_bytes));
+    CU(cudaMemcpyAsync(g.h_stage.p, g.d_out.p, out_bytes, cudaMemcpyDeviceToHost, g.stream));
+    CU(cudaStreamSynchronize(g.stream));
+    const uint8_t *h = (const uint8_t *)g.h_stage.p;
+    memcpy(members, h + o_recs, total * sizeof(b200z_tar_member));
+    for (size_t i = 0; i < n; ++i) memcpy(headers + 512 * at_first[i], h + 512 * cnt[i].first, 512 * cnt[i].count);
+    for (uint64_t k = 0; k < total; ++k)  // zero past a short header (only an archive's last member can have one)
+      if (members[k].header_len < 512) memset(headers + 512 * k + members[k].header_len, 0, 512 - members[k].header_len);
+  }
+  for (size_t i = 0; i < n; ++i) {
+    first[i] = at_first[i];
+    count[i] = cnt[i].count;
+    rc[i] = cnt[i].rc;
+  }
+  *n_total = (size_t)total;
+  return B200Z_OK;
+}
+
+// (test hook, not part of the ABI) the device time of the last b200z_tar_walk_device call's k_tar_walk, by CUDA events
+extern "C" void b200z_debug_tar_walk(double *walk_ms) { *walk_ms = g_tar_walk_ms; }
+
 extern "C" int b200z_zip_extract(const uint8_t *z, size_t len, const b200z_zip_entry *entries, size_t n, uint8_t *out,
                                  size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
                                  int32_t *status, uint32_t flags) {

@@ -1,7 +1,10 @@
 """TAR container: `TarDecoder` / `TarEncoder` / `TarFile`, restated from lib/src/codecs/tar_decoder.dart,
 lib/src/codecs/tar_encoder.dart and lib/src/codecs/tar/tar_file.dart field by field.
 
-The container is host work: one 512-byte header per member, the content sliced out of the tar stream.  The hot path of a
+The container is host work: one 512-byte header per member, the content sliced out of the tar stream.  For archives whose
+members should end up on the GPU, `tar_decode_batch(..., device=...)` and `TarDecoder.decode_bytes(..., device=...)` run
+the member walk there instead (b200z_tar_walk_device): only the headers come back, and each file stays a view into the
+decoded device buffer.  The hot path of a
 tarball is the compression around it, which runs on the device -- `GZipDecoder` / `BZip2Decoder` / `XZDecoder` for one
 tarball, `gzip_decode_batch` / `bzip2_decode_batch` / `xz_decode_batch` for many shards in one call:
 
@@ -15,8 +18,10 @@ the header checksum is never checked; a `././@LongLink` entry names the next mem
 emits V7 headers (no `ustar` magic) and sizes a long-name entry by the name's UTF-16 length."""
 from __future__ import annotations
 
+import ctypes as C
 import re
 
+from . import _ffi
 from ._ffi import E_THROW, DartRangeError
 from .streams import InputFileStream, OutputMemoryStream
 from .zip import Archive, ArchiveFile
@@ -110,8 +115,22 @@ class TarFile:
     @classmethod
     def read(cls, input: _Input, store_data: bool = True) -> "TarFile":
         """TarFile.read (:74-118)."""
+        t = cls.from_header(input.read_bytes(512))  # a short header reads as if the missing bytes were absent fields
+        if store_data or t.filename == LONG_LINK:  # (:104-108)
+            t.raw_content = input.read_bytes(t.file_size)
+        else:
+            input.skip(t.file_size)
+        if t.is_file and t.file_size > 0:  # padding only for "files" with content (:110-117)
+            rem = t.file_size % 512
+            if rem:
+                input.skip(512 - rem)
+        return t
+
+    @classmethod
+    def from_header(cls, h: bytes) -> "TarFile":
+        """The fields TarFile.read parses from a header (:76-103), with no content read.  Header bytes past a short
+        header's end read as absent, whether they are missing or zero."""
         t = cls()
-        h = input.read_bytes(512)  # a short header reads as if the missing bytes were absent fields
         t.filename = _parse_string(h[0:100])
         t.mode = _parse_int(h[100:108])
         t.owner_id = _parse_int(h[108:116])
@@ -131,14 +150,6 @@ class TarFile:
             t.filename_prefix = _parse_string(h[345:500])
             if t.filename_prefix:
                 t.filename = f"{t.filename_prefix}/{t.filename}"
-        if store_data or t.filename == LONG_LINK:  # (:104-108)
-            t.raw_content = input.read_bytes(t.file_size)
-        else:
-            input.skip(t.file_size)
-        if t.is_file and t.file_size > 0:  # padding only for "files" with content (:110-117)
-            rem = t.file_size % 512
-            if rem:
-                input.skip(512 - rem)
         return t
 
     @property
@@ -198,11 +209,27 @@ class TarDecoder:
     def __init__(self):
         self.files: list[TarFile] = []
 
-    def decode_bytes(self, data, verify: bool = False, store_data: bool = True, callback=None) -> Archive:
-        """decodeBytes (:18-22).  `verify` is accepted and ignored, as in the reference."""
+    def decode_bytes(self, data, verify: bool = False, store_data: bool = True, callback=None, device=None) -> Archive:
+        """decodeBytes (:18-22).  `verify` is accepted and ignored, as in the reference.
+
+        device: None walks the members on the host.  The library's torch CUDA device walks them there
+        (b200z_tar_walk_device): `data` is bytes-like (uploaded once) or a 1-D uint8 CUDA tensor (walked where it is), and
+        each file's content is a uint8 tensor view into it -- see tar_decode_batch, of which this is the batch of one.
+        store_data=False raises ValueError with a device: there a negative size moves the walk backwards, which the device
+        walk does not do."""
+        if device is not None:
+            if not store_data:
+                raise ValueError("TarDecoder.decode_bytes: store_data=False has no device walk")
+            from .codecs import _Sink
+            sink = _Sink(device)
+            result = _decode_on_device(sink, _to_device(sink, [data]), [self], callback)[0]
+            if isinstance(result, DartRangeError):
+                raise result
+            return result
         if not isinstance(data, (bytes, bytearray, memoryview)):
             data = bytes(data)
-        return self._decode(_Input(memoryview(data).cast("B")), store_data, callback)
+        inp = _Input(memoryview(data).cast("B"))
+        return self._decode(_host_walk(inp, store_data), store_data, callback)
 
     def decode_stream(self, input, verify: bool = False, store_data: bool = True, callback=None) -> Archive:
         """decodeStream (:24-128) on the rest of an InputMemoryStream or InputFileStream; the stream is left where the walk
@@ -210,25 +237,23 @@ class TarDecoder:
         which throws here for both."""
         if isinstance(input, InputFileStream):
             inp = _Input(input.to_uint8_list())
-            archive = self._decode(inp, store_data, callback)
+            archive = self._decode(_host_walk(inp, store_data), store_data, callback)
             input.skip(inp.pos)
             return archive
         inp = _Input(input.buffer[input.position:])
         try:
-            return self._decode(inp, store_data, callback)
+            return self._decode(_host_walk(inp, store_data), store_data, callback)
         finally:
             input.position += inp.pos
 
-    def _decode(self, input: _Input, store_data: bool, callback) -> Archive:
+    def _decode(self, members, store_data: bool, callback) -> Archive:
+        """The member loop (:28-127) over `members`, the TarFiles of a walk in order, contents read: the host walk
+        (_host_walk) or the records of the device walk (_decode_on_device).  A walk that throws raises from the iterator
+        once the members before the throw are through the loop."""
         archive = Archive()
         self.files = []
         next_name = next_link_name = None
-        data = input.data
-        while not input.is_eos:
-            p = input.pos
-            if len(data) - p < 2 or (data[p] == 0 and data[p + 1] == 0):  # two bytes, not a zero block (:35-38)
-                break
-            tf = TarFile.read(input, store_data)
+        for tf in members:
             if tf.filename == LONG_LINK:  # any type flag, 'K' included (:43-46)
                 raw = tf.raw_content
                 r = raw.find(0)
@@ -273,6 +298,150 @@ class TarDecoder:
             if callback is not None:
                 callback(f)
         return archive
+
+
+def _host_walk(input: _Input, store_data: bool):
+    """The walk of TarDecoder._decode (:28-38): the TarFiles of `input` in order, `input` left where the walk stopped."""
+    data = input.data
+    while not input.is_eos:
+        p = input.pos
+        if len(data) - p < 2 or (data[p] == 0 and data[p + 1] == 0):  # two bytes, not a zero block (:35-38)
+            break
+        yield TarFile.read(input, store_data)
+
+
+_TAR_MEMBER = None  # the numpy dtype of b200z_tar_member
+
+
+def _to_device(sink, shards) -> list:
+    """Archives as 1-D uint8 tensors on the sink's device: CUDA tensors as they are (no copy), everything else (bytes-like,
+    or what bytes() takes) packed into one host buffer and uploaded with one copy."""
+    torch = sink.torch
+    out, host = [None] * len(shards), []
+    for i, s in enumerate(shards):
+        if isinstance(s, torch.Tensor):
+            if s.device != sink.device or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous():
+                raise ValueError(f"tar: shard {i} is not a contiguous 1-D uint8 tensor on {sink.device}")
+            out[i] = s
+        else:  # anything else bytes() takes, as on the host path (a list of ints, ...)
+            host.append((i, memoryview(s if isinstance(s, (bytes, bytearray, memoryview)) else bytes(s)).cast("B")))
+    if host:
+        packed = bytearray(sum(len(v) for _, v in host))
+        at, spans = 0, []
+        for i, v in host:
+            packed[at:at + len(v)] = v
+            spans.append((i, at, len(v)))
+            at += len(v)
+        buf = torch.frombuffer(packed, dtype=torch.uint8).to(sink.device) if packed else \
+            torch.empty(0, dtype=torch.uint8, device=sink.device)
+        for i, a, n in spans:
+            out[i] = buf[a:a + n]
+    return out
+
+
+def _walk_on_device(sink, archives):
+    """One b200z_tar_walk_device call over the archive tensors -> (first, count, rc, records, headers).  The records
+    array starts at a guess of one member per 2 KiB and is sized exactly after an E_NOSPC."""
+    import numpy as np
+    global _TAR_MEMBER
+    if _TAR_MEMBER is None:
+        _TAR_MEMBER = np.dtype([(f, "<u8") for f in ("header_off", "content_off", "content_len")] +
+                               [("size", "<i8"), ("header_len", "<u4"), ("pad_", "<u4")])
+    L = _ffi.ensure_init()
+    n = len(archives)
+    lens = [t.numel() for t in archives]
+    live = [t.data_ptr() for t in archives if t.numel()]
+    base = min(live) if live else 0  # archives from separate allocations: offsets are pointer differences
+    off = (C.c_uint64 * n)(*[t.data_ptr() - base if t.numel() else 0 for t in archives])
+    ln = (C.c_uint64 * n)(*lens)
+    first, count, rc, n_total = (C.c_uint64 * n)(), (C.c_uint64 * n)(), (C.c_int32 * n)(), C.c_size_t()
+    cap = min(sum(x // 512 + 1 for x in lens), sum(lens) // 2048 + n)
+    while True:
+        records, headers = np.empty(max(cap, 1), _TAR_MEMBER), np.empty(max(cap, 1) * 512, np.uint8)
+        r = L.b200z_tar_walk_device(base, off, ln, n, records.ctypes.data, headers.ctypes.data, cap, first, count, rc,
+                                    C.byref(n_total), sink.stream)
+        if r != _ffi.E_NOSPC:
+            _ffi.check(r)
+            return first, count, rc, records, headers
+        cap = n_total.value
+
+
+def _decode_on_device(sink, archives, decoders, callback=None) -> list:
+    """decoders[i]._decode of archives[i] (1-D uint8 tensors on the sink's device) with the walk on the device -> for
+    each, its Archive or the DartRangeError the host walk raises.  The headers are parsed on the host; the contents of
+    LongLink and PAX entries, which the loop reads, come back together in one gather and one copy."""
+    first, count, rc, records, headers = _walk_on_device(sink, archives)
+    members, wanted = [], []
+    for i, t in enumerate(archives):
+        tfs = []
+        for k in range(first[i], first[i] + count[i]):
+            m = records[k]
+            tf = TarFile.from_header(headers[512 * k:512 * k + int(m["header_len"])].tobytes())
+            a, ln = int(m["content_off"]), int(m["content_len"])
+            tf.raw_content = t[a:a + ln]
+            if tf.filename == LONG_LINK or tf.type_flag in (TarFile.EX_HEADER, TarFile.EX_HEADER2):
+                wanted.append(tf)
+            tfs.append(tf)
+        members.append(tfs)
+    if wanted:
+        blob = sink.torch.cat([tf.raw_content for tf in wanted]).cpu().numpy().tobytes()
+        at = 0
+        for tf in wanted:
+            n = tf.raw_content.numel()
+            tf.raw_content, at = blob[at:at + n], at + n
+    out = []
+    for i, (tfs, dec) in enumerate(zip(members, decoders)):
+        try:
+            out.append(dec._decode(_device_members(tfs, rc[i], count[i]), True, callback))
+        except DartRangeError as e:
+            out.append(e)
+    return out
+
+
+def _device_members(tfs, rc, count):
+    yield from tfs
+    if rc == E_THROW:  # the walk stopped at a negative size field: readBytes' RangeError
+        raise DartRangeError(E_THROW, f"tar: negative size field in member {count} (Dart: RangeError)")
+    _ffi.check(rc)
+
+
+def tar_decode_batch(shards, compression=None, verify: bool = False, device=None) -> list:
+    """TarDecoder().decodeBytes of every shard's decoded bytes -> [(rc, Archive or DartRangeError)] in shard order.
+    compression: None (plain .tar), "gzip", "bzip2" or "xz"; the shards are decoded in one codec batch call
+    (gzip_decode_batch, bzip2_decode_batch, xz_decode_batch with `verify`) and rc is that call's rc for the shard (OK for
+    plain shards).  A damaged shard's partial output is walked as it is.  Where TarDecoder would raise DartRangeError for
+    a shard, the error is returned in its place, so one bad shard does not cost the batch.
+
+    device: None decodes and walks on the host side of the library (the recipe
+    `[TarDecoder().decode_bytes(t) for rc, t in gzip_decode_batch(shards)]`).  The library's torch CUDA device decodes
+    straight into device memory (the codec's *_decode_batch_to_device, or one upload of plain shards; plain shards that
+    are already contiguous 1-D uint8 CUDA tensors are walked where they are), walks every member of every shard in one
+    b200z_tar_walk_device call, and gives each file's content as a uint8 tensor view into that memory.  The calls are
+    ordered after torch.cuda.current_stream(), and the tensors are ready when the call returns.  Any other device raises
+    ValueError."""
+    from . import codecs
+    batch = {None: None, "gzip": codecs.gzip_decode_batch, "bzip2": codecs.bzip2_decode_batch, "xz": codecs.xz_decode_batch}
+    if compression not in batch:
+        raise ValueError(f"tar_decode_batch: unknown compression {compression!r}")
+    shards = list(shards)
+    if device is None:
+        decoded = [(_ffi.OK, s) for s in shards] if compression is None else batch[compression](shards, verify=verify)
+        out = []
+        for rc, t in decoded:
+            try:
+                out.append((rc, TarDecoder().decode_bytes(t)))
+            except DartRangeError as e:
+                out.append((rc, e))
+        return out
+    sink = codecs._Sink(device)
+    if not shards:
+        return []
+    if compression is None:
+        decoded = [(_ffi.OK, t) for t in _to_device(sink, shards)]
+    else:
+        decoded = batch[compression](shards, verify=verify, device=sink.device)
+    results = _decode_on_device(sink, [t for _, t in decoded], [TarDecoder() for _ in decoded])
+    return [(rc, r) for (rc, _), r in zip(decoded, results)]
 
 
 class TarEncoder:

@@ -179,6 +179,28 @@ typedef _ZipExtractToDeviceD = int Function(Pointer<Uint8> zip, int zipLen, Poin
     Pointer<Uint8> dOut, int outCap, Pointer<Uint64> outOff, Pointer<Uint64> outRoom, Pointer<Uint64> outLen,
     Pointer<Int32> status, Pointer<Uint32> crc32, int flags, Pointer<Uint8> password, int passwordLen,
     Pointer<Void> cudaStream);
+/// b200z_tar_member (include/b200z.h): one member found by b200z_tar_walk_device.
+final class TarMember extends Struct {
+  @Uint64()
+  external int headerOff;
+  @Uint64()
+  external int contentOff;
+  @Uint64()
+  external int contentLen;
+  @Int64()
+  external int size;
+  @Uint32()
+  external int headerLen;
+  @Uint32()
+  external int pad_;
+}
+
+typedef _TarWalkDeviceC = Int32 Function(Pointer<Uint8> dBase, Pointer<Uint64> off, Pointer<Uint64> len, Size n,
+    Pointer<TarMember> members, Pointer<Uint8> headers, Size cap, Pointer<Uint64> first, Pointer<Uint64> count,
+    Pointer<Int32> rc, Pointer<Size> nTotal, Pointer<Void> cudaStream);
+typedef _TarWalkDeviceD = int Function(Pointer<Uint8> dBase, Pointer<Uint64> off, Pointer<Uint64> len, int n,
+    Pointer<TarMember> members, Pointer<Uint8> headers, int cap, Pointer<Uint64> first, Pointer<Uint64> count,
+    Pointer<Int32> rc, Pointer<Size> nTotal, Pointer<Void> cudaStream);
 typedef _ZipAesEncryptC = Int32 Function(Pointer<Uint8> data, Pointer<Uint64> off, Pointer<Uint64> len, Size n,
     Pointer<Uint8> salts, Pointer<Uint8> password, Size passwordLen, Pointer<Uint8> pwdVerify, Pointer<Uint8> mac);
 typedef _ZipAesEncryptD = int Function(Pointer<Uint8> data, Pointer<Uint64> off, Pointer<Uint64> len, int n,
@@ -302,6 +324,9 @@ class B200Z {
   // dOut: device memory of the library's device; crc32 may be nullptr
   late final _ZipExtractToDeviceD zipExtractToDevice =
       _lib.lookupFunction<_ZipExtractToDeviceC, _ZipExtractToDeviceD>('b200z_zip_extract_to_device');
+  // the TAR member walk over archives in device memory: records and headers come back to the host
+  late final _TarWalkDeviceD tarWalkDevice =
+      _lib.lookupFunction<_TarWalkDeviceC, _TarWalkDeviceD>('b200z_tar_walk_device');
   late final _ZipAesEncryptD zipAesEncrypt = _lib.lookupFunction<_ZipAesEncryptC, _ZipAesEncryptD>('b200z_zip_aes_encrypt');
   late final _Bz2ShardD bzip2DecodeShard = _lib.lookupFunction<_Bz2ShardC, _Bz2ShardD>('b200z_bzip2_decode_shard');
   late final _Crc32D crc32 = _lib.lookupFunction<_Crc32C, _Crc32D>('b200z_crc32');

@@ -336,6 +336,39 @@ int b200z_zip_extract_to_device(const uint8_t *zip, size_t zip_len, const b200z_
                                 size_t out_cap, const uint64_t *out_off, const uint64_t *out_room, uint64_t *out_len,
                                 int32_t *status, uint32_t *crc32, uint32_t flags, const uint8_t *password,
                                 size_t password_len, void *cuda_stream);
+
+/* ---- TAR member walk on the device -----------------------------------------------------------------------------------
+ * b200z_tar_walk_device = the member walk of TarDecoder.decodeBytes(storeData: true) (tar_decoder.dart:28-38,
+ * tar_file.dart:74-118) over n archives already in device memory, d_base[off[i] .. +len[i]).  Each header's size field says
+ * where the next header is, so the walk runs on the device (k_tar_walk, one warp per archive) and only the members' records
+ * and headers come back.  From pos = 0, while pos < len: one byte left, or two zero bytes at pos, end the walk
+ * (OK); the header is the next min(512, len - pos) bytes; `size` is its field at 124..136 as _parseInt reads it (cut at the
+ * first NUL, UTF-8 or else Latin-1, Dart's trim, then [+-]?[0-7]+ or 0); a negative size ends the walk with B200Z_E_THROW
+ * (readBytes' RangeError); the content is the next min(size, what is left) bytes; unless the type byte (156) is '5', a size
+ * that is not a multiple of 512 is padded up to one, clamped to the archive.  Names, links, LongLink and PAX entries do not
+ * move the walk: they are the caller's, read from the headers.
+ *   Memory: d_base is device memory on the b200z_init device; every other array is host memory.
+ *   Results: archive i's members are members[first[i] .. +count[i]), in order, with offsets from the archive's first byte;
+ *     headers[512 k .. +512) is member k's header (zero-filled past header_len); rc[i] is B200Z_OK or B200Z_E_THROW (count[i]
+ *     is then the members before the negative size field); *n_total = the members of all archives.  first[] is the
+ *     exclusive prefix sum of count[]: the layout is archive order, the same on every call.  An archive has at most floor(len[i] / 512) + 1 members, so cap >= sum(floor(len[i] / 512) + 1) always
+ *     suffices.  cap < *n_total: B200Z_E_NOSPC, with *n_total set and nothing else written.
+ *   Argument errors: null arrays (members / headers may be null when cap == 0), wrapping ranges, or an archive whose first or
+ *     last byte is not device memory of the library's device (cudaPointerGetAttributes; archives in separate allocations may
+ *     share d_base through pointer differences, so every archive's range is checked, not d_base alone): B200Z_E_ARG, and
+ *     nothing is written.  n == 0 is OK.  No device: B200Z_E_NODEVICE, nothing is written.
+ *   Ordering: the library's stream waits on an event recorded on cuda_stream (as in the *_decode_batch_to_device calls), and
+ *     the call returns once the results are in place.
+ * One call is two launches whatever n and the member count: k_tar_walk, then one k_copy_slots that gathers the records and
+ * headers into one area, which comes back in one copy.                                                                   */
+typedef struct {
+  uint64_t header_off, content_off, content_len; /* from the archive's first byte; content_len is the clipped read */
+  int64_t size;                                  /* the size field as _parseInt reads it                            */
+  uint32_t header_len, pad_;                     /* 512, fewer when the archive ends inside the header              */
+} b200z_tar_member;
+int b200z_tar_walk_device(const uint8_t *d_base, const uint64_t *off, const uint64_t *len, size_t n, b200z_tar_member *members,
+                          uint8_t *headers, size_t cap, uint64_t *first, uint64_t *count, int32_t *rc, size_t *n_total,
+                          void *cuda_stream);
 /* ZipEncoder(password:) member payloads (zip_encoder.dart:166-183): AES-256 in place on host buffers.  Member i is
  * data[off[i] .. +len[i]) (already compressed), salts[16 i ..] its salt; on return it is the ciphertext,
  * pwd_verify[2 i ..] its password verifier and mac[10 i ..] the first 10 bytes of the HMAC-SHA1 of the ciphertext.  An
